@@ -45,9 +45,12 @@ struct DcnFusedParams {
   int tiles_per_img, num_tiles, kb_per_tap, num_kb;
 };
 
+// What a sample outside the image loads in the gather (eight fp16 zeros, never written).
+__device__ const uint4 g_dcn_zero_tap = {0u, 0u, 0u, 0u};
+
 struct __align__(16) TapEntry {  // 16 bytes: one LDS.128 / STS.128
   int pix;       // (h0*W + w0) of the top-left corner, clamped into the image
-  int step;      // bit0: column neighbour usable, bit1: row neighbour usable
+  int step;      // bit0: column neighbour usable, bit1: row neighbour usable, bit2: the sample is inside the image
   uint32_t w12;  // fp16 pair: corner weights (top-left, top-right), mask folded in
   uint32_t w34;  // fp16 pair: (bottom-left, bottom-right)
 };
@@ -289,9 +292,14 @@ __global__ void __launch_bounds__(kFusedThreads, 1) dcn_fused_kernel(const DcnFu
             const float lh = __fsub_rn(h_im, hf), lw = __fsub_rn(w_im, wf), hh = 1.f - lh, hw = 1.f - lw;
             const bool tp = h_low >= 0, bt = h_low + 1 <= p.H - 1, lf = w_low >= 0, rt = w_low + 1 <= p.W - 1;
             te.pix = max(h_low, 0) * p.W + max(w_low, 0);
-            te.step = ((lf && rt) ? 1 : 0) | ((tp && bt) ? 2 : 0);
+            te.step = ((lf && rt) ? 1 : 0) | ((tp && bt) ? 2 : 0) | 4;
             te.w12 = f2_to_h2((tp && lf) ? hh * hw * m : 0.f, (tp && rt) ? hh * lw * m : 0.f);
             te.w34 = f2_to_h2((bt && lf) ? lh * hw * m : 0.f, (bt && rt) ? lh * lw * m : 0.f);
+          } else {
+            // a sample outside the image is the reference's `0 * mask` whatever the image holds (0 * Inf is NaN): bit 2
+            // of step stays clear and the gather reads a vector of zeros for it, not pixel 0; the first weight keeps the
+            // sign / NaN of the mask
+            te.w12 = f2_to_h2(0.f * m, 0.f);
           }
         }
         table[e] = te;
@@ -316,7 +324,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) dcn_fused_kernel(const DcnFu
         for (int pass = 0; pass < kPasses; ++pass) te[pass] = table[t * kBN + pass * kRowsPerPass + rowp];
 #pragma unroll
         for (int pass = 0; pass < kPasses; ++pass) {
-          const __half *c00 = xb + static_cast<long long>(te[pass].pix) * p.C + cc * kBK + j8 * 8;
+          const __half *c00 = (te[pass].step & 4) ? xb + static_cast<long long>(te[pass].pix) * p.C + cc * kBK + j8 * 8
+                                                  : reinterpret_cast<const __half *>(&g_dcn_zero_tap);
           const int dx = (te[pass].step & 1) ? p.C : 0, dy = (te[pass].step & 2) ? p.W * p.C : 0;
           v[pass][0] = ldg128(c00), v[pass][1] = ldg128(c00 + dx), v[pass][2] = ldg128(c00 + dy),
           v[pass][3] = ldg128(c00 + dy + dx);

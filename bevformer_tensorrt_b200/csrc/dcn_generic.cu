@@ -31,7 +31,7 @@ struct DcnGParams {
 struct DcnTap {
   float w[4];
   int o1;    // offset of the top-left corner inside a channel plane
-  int step;  // bit 0: +1 column usable, bit 1: +1 row usable (W added)
+  int step;  // bit 0: +1 column usable, bit 1: +1 row usable (W added), bit 2: the sample is inside the image
 };
 
 constexpr int kGT = 64;  // tile edge (output channels and pixels)
@@ -108,7 +108,10 @@ __global__ void __launch_bounds__(256) dcn_generic_kernel(const DcnGParams p) {
           tp.w[0] = (ok && tpv && lf) ? hh * hw * m : 0.f, tp.w[1] = (ok && tpv && rt) ? hh * lw * m : 0.f;
           tp.w[2] = (ok && bt && lf) ? lh * hw * m : 0.f, tp.w[3] = (ok && bt && rt) ? lh * lw * m : 0.f;
           tp.o1 = max(h_low, 0) * p.W + max(w_low, 0);
-          tp.step = ((lf && rt) ? 1 : 0) | ((tpv && bt) ? 2 : 0);
+          tp.step = ((lf && rt) ? 1 : 0) | ((tpv && bt) ? 2 : 0) | (ok ? 4 : 0);
+          // a sample outside the image is the reference's `0 * mask`, whatever the image holds: kept in w[0] and
+          // stored as the column value without touching the image
+          if (!ok) tp.w[0] = 0.f * m;
         }
         tab[e] = tp;
       }
@@ -126,8 +129,11 @@ __global__ void __launch_bounds__(256) dcn_generic_kernel(const DcnGParams p) {
       const DcnTap tp = tab[t * kGT + n];
       const T *ip = im + static_cast<long long>(cglob + c) * HW + tp.o1;
       const int dx = tp.step & 1, dy = (tp.step & 2) ? p.W : 0;
-      // corners with weight 0 alias the top-left address (never out of the plane)
-      const float v = fmaf(tp.w[3], g_ld(ip + dy + dx), fmaf(tp.w[2], g_ld(ip + dy), fmaf(tp.w[1], g_ld(ip + dx), tp.w[0] * g_ld(ip))));
+      // A missing corner of a sample inside the image has weight 0 and aliases one of that sample's own in-image corners
+      // (never out of the plane). A sample outside the image reads nothing: its column value is w[0] = 0 * mask.
+      float v = tp.w[0];
+      if (tp.step & 4)
+        v = fmaf(tp.w[3], g_ld(ip + dy + dx), fmaf(tp.w[2], g_ld(ip + dy), fmaf(tp.w[1], g_ld(ip + dx), tp.w[0] * g_ld(ip))));
       Bs[k * kGT + n] = v;
     }
     __syncthreads();

@@ -118,7 +118,9 @@ __global__ void __launch_bounds__(256, INTERP == 2 ? 2 : 4) grid_sample_2d_kerne
       const bool y0 = iy_nw >= 0 && iy_nw < p.Hi, y1 = iy_se >= 0 && iy_se < p.Hi;
       const float w_nw = (x0 && y0) ? fx1 * fy1 : 0.f, w_ne = (x1 && y0) ? fx0 * fy1 : 0.f;
       const float w_sw = (x0 && y1) ? fx1 * fy0 : 0.f, w_se = (x1 && y1) ? fx0 * fy0 : 0.f;
-      // out-of-image taps carry weight 0 and alias an in-image address (clamped), so loads are unconditional
+      // out-of-image taps alias an in-image address (clamped), so loads are unconditional; what they load is dropped
+      // (pk_load_if), not multiplied by their zero weight
+      const bool v_nw = x0 && y0, v_ne = x1 && y0, v_sw = x0 && y1, v_se = x1 && y1;
       const int cx0 = min(max(ix_nw, 0), p.Wi - 1), cx1 = min(max(ix_se, 0), p.Wi - 1);
       const int cy0 = min(max(iy_nw, 0), p.Hi - 1), cy1 = min(max(iy_se, 0), p.Hi - 1);
       const int o_nw = cy0 * p.Wi + cx0, o_ne = cy0 * p.Wi + cx1, o_sw = cy1 * p.Wi + cx0, o_se = cy1 * p.Wi + cx1;
@@ -127,8 +129,8 @@ __global__ void __launch_bounds__(256, INTERP == 2 ? 2 : 4) grid_sample_2d_kerne
 #pragma unroll 8
       for (int cp = cp0; cp < cp1; ++cp, ip += plane_i, op += plane_o) {
         float a[W], b[W], c[W], d[W], o[W];
-        P::load(ip + o_nw, a, p.scale_i), P::load(ip + o_ne, b, p.scale_i);
-        P::load(ip + o_sw, c, p.scale_i), P::load(ip + o_se, d, p.scale_i);
+        pk_load_if<K>(ip + o_nw, v_nw, a, p.scale_i), pk_load_if<K>(ip + o_ne, v_ne, b, p.scale_i);
+        pk_load_if<K>(ip + o_sw, v_sw, c, p.scale_i), pk_load_if<K>(ip + o_se, v_se, d, p.scale_i);
 #pragma unroll
         for (int i = 0; i < W; ++i) o[i] = fmaf(d[i], w_se, fmaf(c[i], w_sw, fmaf(b[i], w_ne, a[i] * w_nw)));
         P::store(op, o, so);
@@ -242,6 +244,7 @@ __global__ void __launch_bounds__(256, 4) grid_sample_2d_tile_kernel(const GsPar
   const float so = K == kI8x4 ? 1.f / p.scale_o : 1.f;
 
   float w_nw = 0.f, w_ne = 0.f, w_sw = 0.f, w_se = 0.f;
+  bool v_nw = false, v_ne = false, v_sw = false, v_se = false;  // tap inside the image
   int cx0 = INT_MAX, cx1 = INT_MIN, cy0 = INT_MAX, cy1 = INT_MIN;
   if (valid) {
     float gx, gy, gz;
@@ -256,7 +259,8 @@ __global__ void __launch_bounds__(256, 4) grid_sample_2d_tile_kernel(const GsPar
     const bool y0 = iy_nw >= 0 && iy_nw < p.Hi, y1 = iy_se >= 0 && iy_se < p.Hi;
     w_nw = (x0 && y0) ? fx1 * fy1 : 0.f, w_ne = (x1 && y0) ? fx0 * fy1 : 0.f;
     w_sw = (x0 && y1) ? fx1 * fy0 : 0.f, w_se = (x1 && y1) ? fx0 * fy0 : 0.f;
-    // out-of-image taps carry weight 0 and alias an in-image pixel (clamped), so loads are unconditional
+    // out-of-image taps alias an in-image pixel (clamped), so loads are unconditional; what they load is dropped
+    v_nw = x0 && y0, v_ne = x1 && y0, v_sw = x0 && y1, v_se = x1 && y1;
     cx0 = min(max(ix_nw, 0), p.Wi - 1), cx1 = min(max(ix_se, 0), p.Wi - 1);
     cy0 = min(max(iy_nw, 0), p.Hi - 1), cy1 = min(max(iy_se, 0), p.Hi - 1);
   }
@@ -336,8 +340,8 @@ __global__ void __launch_bounds__(256, 4) grid_sample_2d_tile_kernel(const GsPar
         if (c >= ncp) break;
         const T *wc = win + c * (kBH * RE);
         float a[W], b[W], cc[W], d[W], o[W];
-        P::unpack(wc[o_nw], a, p.scale_i), P::unpack(wc[o_ne], b, p.scale_i);
-        P::unpack(wc[o_sw], cc, p.scale_i), P::unpack(wc[o_se], d, p.scale_i);
+        pk_unpack_if<K>(wc[o_nw], v_nw, a, p.scale_i), pk_unpack_if<K>(wc[o_ne], v_ne, b, p.scale_i);
+        pk_unpack_if<K>(wc[o_sw], v_sw, cc, p.scale_i), pk_unpack_if<K>(wc[o_se], v_se, d, p.scale_i);
 #pragma unroll
         for (int i = 0; i < W; ++i) o[i] = fmaf(d[i], w_se, fmaf(cc[i], w_sw, fmaf(b[i], w_ne, a[i] * w_nw)));
         P::store(out_p + c * plane_o, o, so);
@@ -350,8 +354,8 @@ __global__ void __launch_bounds__(256, 4) grid_sample_2d_tile_kernel(const GsPar
 #pragma unroll 4
     for (int cp = cp0; cp < cp1; ++cp, ip += plane_i, op += plane_o) {
       float a[W], b[W], cc[W], d[W], o[W];
-      P::load(ip + o_nw, a, p.scale_i), P::load(ip + o_ne, b, p.scale_i);
-      P::load(ip + o_sw, cc, p.scale_i), P::load(ip + o_se, d, p.scale_i);
+      pk_load_if<K>(ip + o_nw, v_nw, a, p.scale_i), pk_load_if<K>(ip + o_ne, v_ne, b, p.scale_i);
+      pk_load_if<K>(ip + o_sw, v_sw, cc, p.scale_i), pk_load_if<K>(ip + o_se, v_se, d, p.scale_i);
 #pragma unroll
       for (int i = 0; i < W; ++i) o[i] = fmaf(d[i], w_se, fmaf(cc[i], w_sw, fmaf(b[i], w_ne, a[i] * w_nw)));
       P::store(op, o, so);
@@ -386,6 +390,7 @@ __global__ void __launch_bounds__(256) grid_sample_3d_kernel(const GsParams p) {
       const float fx = ix - x0, fy = iy - y0, fz = iz - z0;
       int off[8];
       float wt[8];
+      unsigned inside = 0;  // bit t: corner t is inside the volume
 #pragma unroll
       for (int t = 0; t < 8; ++t) {
         const int dx = t & 1, dy = (t >> 1) & 1, dz = t >> 2;
@@ -398,13 +403,14 @@ __global__ void __launch_bounds__(256) grid_sample_3d_kernel(const GsParams p) {
         const float wz = dz ? fz : (static_cast<float>(z0 + 1) - iz);
         wt[t] = ok ? wx * wy * wz : 0.f;
         off[t] = ok ? (z * p.Hi + y) * p.Wi + x : 0;
+        inside |= ok ? 1u << t : 0u;
       }
       for (int cp = cp0; cp < cp1; ++cp, ip += plane_i, op += plane_o) {
         float o[1] = {0.f};
 #pragma unroll
         for (int t = 0; t < 8; ++t) {
           float v[1];
-          P::load(ip + off[t], v, 1.f);
+          pk_load_if<K>(ip + off[t], (inside >> t) & 1u, v, 1.f);  // an outside corner reads element 0 and drops it
           o[0] = fmaf(v[0], wt[t], o[0]);
         }
         P::store(op, o, 1.f);

@@ -404,6 +404,9 @@ struct RefRaw<float> {
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kMaxChunks = 64;
 
+// What a sampling point outside every image loads in the gather kernel (one tap vector of zeros, never written).
+__device__ const uint4 g_msda_zero_tap = {0u, 0u, 0u, 0u};
+
 //
 // UPW ("units per warp", plugin-op form EPI = 0 only) > 1 is the batched launch: a CTA covers UPW consecutive blocks of
 // IPB items and each warp walks UPW units (unit u of warp w = the 32/LPI items at item0 + u*IPB + w*IPW, the same item
@@ -665,6 +668,7 @@ __global__ void __launch_bounds__(NT, MINB) msda_gather_kernel(const MsdaParams 
   }
 
   // ---- phase C: gather
+  const char *zeros = reinterpret_cast<const char *>(&g_msda_zero_tap);
   const unsigned step_b = static_cast<unsigned>(M * C) * sizeof(T);  // bytes between horizontally adjacent pixels
   const char *vbase = reinterpret_cast<const char *>(static_cast<const T *>(prm.value) +
                                                      (static_cast<long long>(b) * prm.S * M + m) * C + sub * VEC);
@@ -691,7 +695,7 @@ __global__ void __launch_bounds__(NT, MINB) msda_gather_kernel(const MsdaParams 
         const int h0 = max(h_low, 0), w0 = max(w_low, 0);
         const bool t = h_low >= 0, bt = h_low + 1 <= H - 1, lf = w_low >= 0, rt = w_low + 1 <= W - 1;
         const unsigned top = ok ? static_cast<unsigned>(start + h0 * W + w0) * step_b : 0u;
-        otop[k] = top | ((ok && lf && rt) ? 1u : 0u);
+        otop[k] = top | ((ok && lf && rt) ? 1u : 0u) | (ok ? 2u : 0u);  // tap offsets are multiples of 16 bytes
         obot[k] = top + ((ok && t && bt) ? static_cast<unsigned>(W) * step_b : 0u);
         const float hh = 1.f - lh, hw = 1.f - lw;
         const float e = EPI == 2 ? lg[r][k] * mk : lg[r][k];  // bev_mask folded into the tap weights
@@ -724,8 +728,9 @@ __global__ void __launch_bounds__(NT, MINB) msda_gather_kernel(const MsdaParams 
 #pragma unroll
             for (int n = 0; n < NW; ++n) wp[i][n] = __shfl_sync(kFullMask, tw[k0 + i][n], src);
             const unsigned dx = (ot & 1u) ? step_b : 0u;
-            const char *p0 = vbase + (ot & ~1u);
-            const char *p1 = vbase + ob;
+            const char *base = (ot & 2u) ? vbase : zeros;  // see the note at the one-point form below
+            const char *p0 = base + (ot & ~3u);
+            const char *p1 = base + ob;
             tp[i][0] = IO::ld(p0), tp[i][1] = IO::ld(p0 + dx), tp[i][2] = IO::ld(p1), tp[i][3] = IO::ld(p1 + dx);
           }
 #pragma unroll
@@ -740,11 +745,15 @@ __global__ void __launch_bounds__(NT, MINB) msda_gather_kernel(const MsdaParams 
         float w[NW];
 #pragma unroll
         for (int i = 0; i < NW; ++i) w[i] = __shfl_sync(kFullMask, tw[k][i], src);
-        // Taps of a point whose neighbour is outside the image alias an in-image tap and carry weight 0; points that
-        // are out of range altogether read the (valid) first bytes of this item's slice with all-zero weights.
+        // A point in range whose neighbour is outside the image: the missing taps carry weight 0 and alias one of the
+        // point's own in-image taps, so they add nothing that tap does not add already. A point out of range altogether
+        // (bit 1 of ot clear; its offsets and weights are all 0) has no tap of its own to alias, and no element of value
+        // may be assumed finite (0 * Inf is NaN): it reads 16 bytes of zeros instead, so it adds an exact 0 and the loop
+        // stays free of branches.
         const unsigned dx = (ot & 1u) ? step_b : 0u;
-        const char *p0 = vbase + (ot & ~1u);
-        const char *p1 = vbase + ob;
+        const char *base = (ot & 2u) ? vbase : zeros;
+        const char *p0 = base + (ot & ~3u);
+        const char *p1 = base + ob;
         const typename IO::Tap t[4] = {IO::ld(p0), IO::ld(p0 + dx), IO::ld(p1), IO::ld(p1 + dx)};
         IO::fma_point(acc, t, w);
       }

@@ -243,6 +243,7 @@ __global__ void __launch_bounds__(kResThreads, 1) msda_res_kernel(const ResParam
         const int Wc = __shfl_sync(kFullMask, lvW, lvc);
         const int startc = __shfl_sync(kFullMask, lvStart, lvc);
         unsigned pa[4], pb[4];
+        const unsigned inp = __shfl_sync(kFullMask, inr, src);  // the owner's range bits of this chunk's four points
         float wt[4], wb[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -250,7 +251,8 @@ __global__ void __launch_bounds__(kResThreads, 1) msda_res_kernel(const ResParam
           const float w0 = __shfl_sync(kFullMask, tw[k][0], src), w1 = __shfl_sync(kFullMask, tw[k][1], src);
           const float w2 = __shfl_sync(kFullMask, tw[k][2], src), w3 = __shfl_sync(kFullMask, tw[k][3], src);
           wt[k] = col ? w1 : w0, wb[k] = col ? w3 : w2;
-          // neighbours outside the image alias an in-image tap and carry weight 0
+          // a neighbour outside the image carries weight 0 and aliases one of the point's own in-image taps; a point
+          // out of range altogether (bit k of inp clear) aliases the level's first pixel and is left out of the sum
           pa[k] = (cd >> 2) + (static_cast<unsigned>(col) & cd & 1u);
           pb[k] = pa[k] + ((cd & 2u) ? static_cast<unsigned>(Wc) : 0u);
         }
@@ -270,6 +272,7 @@ __global__ void __launch_bounds__(kResThreads, 1) msda_res_kernel(const ResParam
         }
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
+          if (!((inp >> k) & 1u)) continue;
           fma8(acc, va[k], wt[k]);
           fma8(acc, vb[k], wb[k]);
         }

@@ -10,6 +10,10 @@ namespace b200 {
 
 enum { kF32 = 0, kF16 = 1, kF16x2 = 2, kI8x4 = 3 };
 
+// Pk<K>::zero() is the packet whose every channel unpacks to +0. A bilinear tap outside the image is loaded from a
+// clamped (in-image) address and then replaced by it (pk_load_if), so that it contributes exactly 0 whatever the
+// aliased pixel holds: 0 * Inf and 0 * NaN are NaN, and the reference never loads such a tap at all.
+
 template <int K>
 struct Pk;
 template <>
@@ -18,6 +22,7 @@ struct Pk<kF32> {
   static constexpr int W = 1;
   __device__ static void unpack(T raw, float (&v)[1], float) { v[0] = raw; }
   __device__ static void load(const T *p, float (&v)[1], float) { v[0] = __ldg(p); }
+  __device__ static T zero() { return 0.f; }
   __device__ static void store(T *p, const float (&v)[1], float) { *p = v[0]; }
   __device__ static void grid_xy(const void *g, long long plane, long long pix, long long n, float, float &x, float &y,
                                  float &z, bool has_z) {
@@ -31,6 +36,7 @@ struct Pk<kF16> {
   static constexpr int W = 1;
   __device__ static void unpack(T raw, float (&v)[1], float) { v[0] = __half2float(raw); }
   __device__ static void load(const T *p, float (&v)[1], float) { v[0] = __half2float(__ldg(p)); }
+  __device__ static T zero() { return __ushort_as_half(0); }
   __device__ static void store(T *p, const float (&v)[1], float) { *p = __float2half_rn(v[0]); }
   __device__ static void grid_xy(const void *g, long long plane, long long pix, long long n, float, float &x, float &y,
                                  float &z, bool has_z) {
@@ -51,6 +57,7 @@ struct Pk<kF16x2> {  // kCHW2: [N, ceil(C/2), H, W, 2]; the 2-channel grid is on
     const float2 f = h2_to_f2(__ldg(p));
     v[0] = f.x, v[1] = f.y;
   }
+  __device__ static T zero() { return 0u; }
   __device__ static void store(T *p, const float (&v)[2], float) { *p = f2_to_h2(v[0], v[1]); }
   __device__ static void grid_xy(const void *g, long long plane, long long pix, long long n, float, float &x, float &y,
                                  float &z, bool) {
@@ -71,6 +78,7 @@ struct Pk<kI8x4> {  // kCHW4: [N, ceil(C/4), H, W, 4]; grid = (x, y, pad, pad) i
 #pragma unroll
     for (int i = 0; i < 4; ++i) v[i] = static_cast<float>(static_cast<int8_t>(u >> (8 * i))) * s;
   }
+  __device__ static T zero() { return 0u; }
   __device__ static void store(T *p, const float (&v)[4], float inv_so) {
     uint32_t u = 0;
 #pragma unroll
@@ -84,5 +92,14 @@ struct Pk<kI8x4> {  // kCHW4: [N, ceil(C/4), H, W, 4]; grid = (x, y, pad, pad) i
     z = 0.f;
   }
 };
+
+template <int K>
+__device__ __forceinline__ void pk_unpack_if(typename Pk<K>::T raw, bool valid, float (&v)[Pk<K>::W], float s) {
+  Pk<K>::unpack(valid ? raw : Pk<K>::zero(), v, s);  // one select on the raw word, before any conversion
+}
+template <int K>
+__device__ __forceinline__ void pk_load_if(const typename Pk<K>::T *p, bool valid, float (&v)[Pk<K>::W], float s) {
+  pk_unpack_if<K>(__ldg(p), valid, v, s);
+}
 
 }  // namespace b200

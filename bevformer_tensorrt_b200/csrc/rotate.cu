@@ -78,10 +78,13 @@ __device__ __forceinline__ void rot_source_index(const float (&m)[4], int w, int
   iy = rot_safe(__fmul_rn(__fmaf_rn(static_cast<float>(H), __fadd_rn(gy, 1.f), -1.f), 0.5f));
 }
 
-// Four taps of one output pixel: clamped offsets (in pixels) and weights (0 for out-of-image taps). Nearest = one tap.
+// Four taps of one output pixel: clamped offsets (in pixels), weights and validity (bit i of `in`: tap i is inside the
+// image). An out-of-image tap aliases an in-image pixel; what it loads is dropped, not multiplied by its zero weight
+// (0 * Inf is NaN, and the reference never loads such a tap). Nearest = one tap.
 struct RotTaps {
   int o[4];
   float w[4];
+  unsigned in;
 };
 template <int INTERP>
 __device__ __forceinline__ RotTaps rot_taps(float ix, float iy, int W, int H) {
@@ -97,11 +100,13 @@ __device__ __forceinline__ RotTaps rot_taps(float ix, float iy, int W, int H) {
     const int cx0 = min(max(x0, 0), W - 1), cx1 = min(max(x1, 0), W - 1);
     const int cy0 = min(max(y0, 0), H - 1), cy1 = min(max(y1, 0), H - 1);
     t.o[0] = cy0 * W + cx0, t.o[1] = cy0 * W + cx1, t.o[2] = cy1 * W + cx0, t.o[3] = cy1 * W + cx1;
+    t.in = ((vx0 && vy0) ? 1u : 0u) | ((vx1 && vy0) ? 2u : 0u) | ((vx0 && vy1) ? 4u : 0u) | ((vx1 && vy1) ? 8u : 0u);
   } else {
     const int xn = static_cast<int>(roundf(ix)), yn = static_cast<int>(roundf(iy));  // ::round (:190-191)
     const bool ok = xn >= 0 && xn < W && yn >= 0 && yn < H;
     t.o[0] = ok ? yn * W + xn : 0, t.w[0] = ok ? 1.f : 0.f;
     t.o[1] = t.o[2] = t.o[3] = 0, t.w[1] = t.w[2] = t.w[3] = 0.f;
+    t.in = ok ? 1u : 0u;
   }
   return t;
 }
@@ -137,8 +142,8 @@ __global__ void __launch_bounds__(256, 4) rotate_planar_kernel(const RotParams p
 #pragma unroll 4
       for (int cp = cp0; cp < cp1; ++cp, ip += plane, op += plane) {
         float a[PW], b[PW], c[PW], d[PW], o[PW];
-        P::load(ip + t.o[0], a, p.scale_i), P::load(ip + t.o[1], b, p.scale_i);
-        P::load(ip + t.o[2], c, p.scale_i), P::load(ip + t.o[3], d, p.scale_i);
+        pk_load_if<K>(ip + t.o[0], t.in & 1u, a, p.scale_i), pk_load_if<K>(ip + t.o[1], t.in & 2u, b, p.scale_i);
+        pk_load_if<K>(ip + t.o[2], t.in & 4u, c, p.scale_i), pk_load_if<K>(ip + t.o[3], t.in & 8u, d, p.scale_i);
 #pragma unroll
         for (int i = 0; i < PW; ++i)
           o[i] = fmaf(d[i], t.w[3], fmaf(c[i], t.w[2], fmaf(b[i], t.w[1], a[i] * t.w[0])));
@@ -163,8 +168,9 @@ struct Vec16;
 template <>
 struct Vec16<kF32> {
   static constexpr int N = 4;
-  __device__ static void load(const void *p, float (&v)[4]) {
-    const uint4 u = ldg128(p);
+  __device__ static void load(const void *p, bool valid, float (&v)[4]) {
+    uint4 u = ldg128(p);
+    if (!valid) u = make_uint4(0u, 0u, 0u, 0u);
     v[0] = __uint_as_float(u.x), v[1] = __uint_as_float(u.y), v[2] = __uint_as_float(u.z), v[3] = __uint_as_float(u.w);
   }
   __device__ static void store(void *p, const float (&v)[4]) {
@@ -175,8 +181,9 @@ struct Vec16<kF32> {
 template <>
 struct Vec16<kF16> {
   static constexpr int N = 8;
-  __device__ static void load(const void *p, float (&v)[8]) {
-    const uint4 u = ldg128(p);
+  __device__ static void load(const void *p, bool valid, float (&v)[8]) {
+    uint4 u = ldg128(p);
+    if (!valid) u = make_uint4(0u, 0u, 0u, 0u);
     const uint32_t r[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -224,13 +231,12 @@ __global__ void __launch_bounds__(256, 3) rotate_hwc_kernel(const RotParams p) {
       float o[N];
       if (INTERP == 0) {
         float a[N], b[N], c[N], d[N];
-        V::load(i0 + off, a), V::load(i1 + off, b), V::load(i2 + off, c), V::load(i3 + off, d);
+        V::load(i0 + off, t.in & 1u, a), V::load(i1 + off, t.in & 2u, b), V::load(i2 + off, t.in & 4u, c);
+        V::load(i3 + off, t.in & 8u, d);
 #pragma unroll
         for (int i = 0; i < N; ++i) o[i] = fmaf(d[i], t.w[3], fmaf(c[i], t.w[2], fmaf(b[i], t.w[1], a[i] * t.w[0])));
       } else {
-        V::load(i0 + off, o);
-#pragma unroll
-        for (int i = 0; i < N; ++i) o[i] = t.w[0] != 0.f ? o[i] : 0.f;
+        V::load(i0 + off, t.in & 1u, o);
       }
       V::store(op + off, o);
     }
