@@ -35,8 +35,8 @@ constexpr int kMinBlocks = B200_MSDA_MIN_BLOCKS;  // 3: registers capped at 85, 
 // exact by default; 1 = mixed FHFMA (opt-in, see Io<__half, 1>). Atomic: enqueue may be called from several host
 // threads (SURVEY §8(b) threading), the setter from another.
 static std::atomic<int> g_f16_mode{0};
-// FP16 kernel selection: 1 (default) = resident-tail kernel (msda_res.cu) where its envelope holds, 0 = this file's
-// round-1 gather kernel everywhere.
+// FP16 kernel selection: 0 (default) = this file's round-1 gather kernel everywhere, 1 (opt-in, measured slower) =
+// resident-tail kernel (msda_res.cu) where its envelope holds.
 static std::atomic<int> g_f16_path{0};
 static std::atomic<int> g_res_cap_bytes{128 * 1024};
 // Launch shape of the FP32 / FP16 plugin op, encoded as units | strided << 8. units: 1 = one block of items per CTA

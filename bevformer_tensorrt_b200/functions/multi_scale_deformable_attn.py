@@ -415,7 +415,10 @@ def multi_scale_deformable_attn_sca_shared(value, value_spatial_shapes, referenc
         sampling_offsets [1 | -, nq, heads, L*P*2], attention_weights [1 | -, nq, heads, L*P]
 
     Returns slots float32 [nq, heads*ch] = sum_b bev_mask[b] * MSDA(value[b], ref[b], offsets, logits), every element
-    written exactly once (one item per (query, head), cameras looped in registers, softmax evaluated once)."""
+    written exactly once (one item per (query, head), cameras looped in registers, softmax evaluated once). Shapes the
+    fused kernel does not take (more than two gather rounds, channels != 32, G not in {1, 2, 4}, P % 4 != 0, unaligned
+    tensors) run the plugin op on ``bs`` copies of offsets / logits and sum the masked cameras, like
+    ``multi_scale_deformable_attn_sca``."""
     if not value.is_cuda:
         raise RuntimeError("multi_scale_deformable_attn_sca_shared: value must be a CUDA tensor (no CPU fallback exists)")
     if value.dim() != 4:
@@ -450,6 +453,12 @@ def multi_scale_deformable_attn_sca_shared(value, value_spatial_shapes, referenc
                                 mask.data_ptr(), bs, num_keys, num_heads, channels, num_levels, num_query,
                                 all_points // num_levels, points_per_group, slots.data_ptr(),
                                 _lib.current_stream_ptr())  # fmt: skip
+        if st == 1:
+            # shapes the fused kernel does not take: plugin op on bs copies of offsets / logits + masked camera sum
+            rep_off = off.reshape(1, num_query, num_heads, all_points * 2).expand(bs, -1, -1, -1)
+            rep_w = w.reshape(1, num_query, num_heads, all_points).expand(bs, -1, -1, -1)
+            out = _msda_forward(value, shapes, ref, rep_off, rep_w, False)
+            return (out.reshape(bs, num_query, -1).float() * mask.unsqueeze(-1)).sum(0)
     _lib.check(name, st)
     return slots
 

@@ -57,7 +57,7 @@ def _oracle_f32(inputs):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# resident-tail FP16 kernel (csrc/msda_res.cu): the library default behind the FP16 plugin op
+# resident-tail FP16 kernel (csrc/msda_res.cu): opt-in behind the FP16 plugin op (set_msda_f16_path(True))
 # ---------------------------------------------------------------------------------------------------------------
 RES_EXTRA = {
     # more (batch, head) pairs than SMs: CTAs walk several pairs and re-stage the tail in between
@@ -753,6 +753,10 @@ def test_shared_sca_matches_masked_camera_sum_of_oracle(name, dist, dtype, tol):
 
 
 def test_shared_sca_base_shapes_and_errors():
+    """BASELINE configs[2]: inside the fused kernel's envelope the camera-shared op is ONE launch (no memset, no
+    fallback) and agrees with the per-camera fused op on the repeated tensors. Shapes outside the envelope take the
+    plugin op + masked camera sum instead (tests/test_msda_envelope_gpu.py). Repeated offsets / logits and CPU tensors
+    are refused."""
     from bevformer_tensorrt_b200.workloads import bev_reference_points_cam, camera_ring_lidar2img
 
     cfg = CONFIGS["base_sca"]
