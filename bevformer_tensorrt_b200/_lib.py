@@ -141,6 +141,19 @@ def check(fn_name: str, status: int) -> None:
         raise B200OpsError(fn_name, status)
 
 
+def call(fn_name: str, device, *args, accept=(B200_OK,)) -> int:
+    """Calls the C entry ``fn_name`` with ``args`` followed by the current stream of ``device``, with ``device`` made
+    the current device, and returns its status. A status outside ``accept`` raises B200OpsError; callers that fall back
+    on B200_ERR_UNSUPPORTED pass ``accept=(0, 1)``."""
+    import torch
+
+    with torch.cuda.device(device):
+        status = getattr(load(), fn_name)(*args, current_stream_ptr())
+    if status not in accept:
+        raise B200OpsError(fn_name, status)
+    return status
+
+
 def launch_count() -> int:
     return int(load().b200_launch_count())
 

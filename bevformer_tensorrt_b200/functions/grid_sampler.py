@@ -28,18 +28,15 @@ def _dims(t):
 
 
 def _launch(name, out, inp, grid, out_shape, in_shape, grid_shape, mode, pad, align, scales=None):
-    lib = _lib.load()
     nb = len(in_shape)
     od, idm, gd = ((ctypes.c_int * nb)(*s) for s in (out_shape, in_shape, grid_shape))
-    with torch.cuda.device(inp.device):
-        if scales is None:
-            st = getattr(lib, name)(out.data_ptr(), inp.data_ptr(), grid.data_ptr(), od, idm, gd, nb, mode, pad,
-                                    int(bool(align)), _lib.current_stream_ptr())  # fmt: skip
-        else:
-            so, si, sg = scales
-            st = getattr(lib, name)(out.data_ptr(), float(so), inp.data_ptr(), float(si), grid.data_ptr(), float(sg),
-                                    od, idm, gd, nb, mode, pad, int(bool(align)), _lib.current_stream_ptr())  # fmt: skip
-    _lib.check(name, st)
+    if scales is None:
+        _lib.call(name, inp.device, out.data_ptr(), inp.data_ptr(), grid.data_ptr(), od, idm, gd, nb, mode, pad,
+                  int(bool(align)))  # fmt: skip
+    else:
+        so, si, sg = scales
+        _lib.call(name, inp.device, out.data_ptr(), float(so), inp.data_ptr(), float(si), grid.data_ptr(), float(sg),
+                  od, idm, gd, nb, mode, pad, int(bool(align)))  # fmt: skip
     return out
 
 

@@ -17,6 +17,11 @@ from torch.nn.modules.utils import _pair
 from .. import _lib
 
 
+def _out_extent(size, kernel, stride, padding, dilation):
+    """Output length of a convolution along one axis."""
+    return (size + 2 * padding - (dilation * (kernel - 1) + 1)) // stride + 1
+
+
 def _forward(input, offset, mask, weight, bias, stride, padding, dilation, groups, deform_groups):
     if not input.is_cuda:
         raise RuntimeError("modulated_deformable_conv2d: input must be a CUDA tensor (no CPU fallback exists)")
@@ -30,8 +35,7 @@ def _forward(input, offset, mask, weight, bias, stride, padding, dilation, group
     co, cig, kh, kw = weight.shape
     if cig * groups != c:
         raise ValueError("weight.shape[1] * groups must equal the input channels")
-    ho = (h + 2 * ph - (dh * (kh - 1) + 1)) // sh + 1
-    wo = (w + 2 * pw - (dw * (kw - 1) + 1)) // sw + 1
+    ho, wo = _out_extent(h, kh, sh, ph, dh), _out_extent(w, kw, sw, pw, dw)
     if tuple(offset.shape) != (n, deform_groups * 2 * kh * kw, ho, wo):
         raise ValueError(f"offset must be {(n, deform_groups * 2 * kh * kw, ho, wo)}, got {tuple(offset.shape)}")
     if tuple(mask.shape) != (n, deform_groups * kh * kw, ho, wo):
@@ -47,12 +51,10 @@ def _forward(input, offset, mask, weight, bias, stride, padding, dilation, group
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=input.device)
     out = torch.empty(n, co, ho, wo, dtype=dt, device=input.device)
     name = "b200_dcn_f32" if dt == torch.float32 else "b200_dcn_f16"
-    with torch.cuda.device(input.device):
-        st = getattr(lib, name)(input.data_ptr(), weight.data_ptr(), bias_t.data_ptr() if bias_t is not None else None,
-                                offset.data_ptr(), mask.data_ptr(), out.data_ptr(), workspace.data_ptr(), n, c, h, w,
-                                co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups, min(n, 32), None,
-                                _lib.current_stream_ptr())  # fmt: skip
-    _lib.check(name, st)
+    _lib.call(name, input.device, input.data_ptr(), weight.data_ptr(),
+              bias_t.data_ptr() if bias_t is not None else None, offset.data_ptr(), mask.data_ptr(), out.data_ptr(),
+              workspace.data_ptr(), n, c, h, w, co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups, min(n, 32),
+              None)  # fmt: skip
     return out
 
 
@@ -62,10 +64,7 @@ _PACKED = {}  # id(weight) -> (weakref to the weight, its _version, packed copy)
 def _pack(lib, weight):
     co, c, kh, kw = weight.shape
     packed = torch.empty_like(weight, memory_format=torch.contiguous_format)
-    with torch.cuda.device(weight.device):
-        _lib.check("b200_dcn_pack_weights_f16",
-                   lib.b200_dcn_pack_weights_f16(weight.data_ptr(), packed.data_ptr(), co, c, kh, kw,
-                                                 _lib.current_stream_ptr()))  # fmt: skip
+    _lib.call("b200_dcn_pack_weights_f16", weight.device, weight.data_ptr(), packed.data_ptr(), co, c, kh, kw)
     return packed
 
 
@@ -108,12 +107,10 @@ def _forward_fused_f16(lib, input, offset, mask, weight, bias, stride, padding, 
                                            dilation[1], dilation[0])  # fmt: skip
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=input.device)
     out = torch.empty(n, co, out_hw[0], out_hw[1], dtype=dt, device=input.device)
-    with torch.cuda.device(input.device):
-        st = lib.b200_dcn_f16_ex(x.data_ptr(), wp.data_ptr(), bias_t.data_ptr() if bias_t is not None else None,
-                                 offset.data_ptr(), mask.data_ptr(), out.data_ptr(), workspace.data_ptr(), n, c, h, w, co,
-                                 kw, kh, stride[1], stride[0], padding[1], padding[0], dilation[1], dilation[0], 1, 1,
-                                 flags, _lib.current_stream_ptr())  # fmt: skip
-    _lib.check("b200_dcn_f16_ex", st)
+    _lib.call("b200_dcn_f16_ex", input.device, x.data_ptr(), wp.data_ptr(),
+              bias_t.data_ptr() if bias_t is not None else None, offset.data_ptr(), mask.data_ptr(), out.data_ptr(),
+              workspace.data_ptr(), n, c, h, w, co, kw, kh, stride[1], stride[0], padding[1], padding[0], dilation[1],
+              dilation[0], 1, 1, flags)  # fmt: skip
     return out
 
 
@@ -139,11 +136,8 @@ def _backward(grad_out, input, offset, mask, weight, bias, stride, padding, dila
     ptr = [g.data_ptr() if g is not None else None for g in grads]
     name = "b200_dcn_backward_f32" if dt == torch.float32 else "b200_dcn_backward_f16"
     flags = [] if dt == torch.float32 else [0]
-    with torch.cuda.device(x.device):
-        st = getattr(lib, name)(x.data_ptr(), wt.data_ptr(), off.data_ptr(), msk.data_ptr(), go.data_ptr(), *ptr,
-                                workspace.data_ptr(), n, c, h, w, co, kw, kh, sw, sh, pw, ph, dw, dh, groups,
-                                deform_groups, *flags, _lib.current_stream_ptr())  # fmt: skip
-    _lib.check(name, st)
+    _lib.call(name, x.device, x.data_ptr(), wt.data_ptr(), off.data_ptr(), msk.data_ptr(), go.data_ptr(), *ptr,
+              workspace.data_ptr(), n, c, h, w, co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups, *flags)
     gi, gw, gb, go_, gm = grads
     cast = lambda g, t: g.to(t.dtype) if g is not None else None  # noqa: E731
     return cast(gi, input), cast(go_, offset), cast(gm, mask), cast(gw, weight), cast(gb, bias)
@@ -201,20 +195,17 @@ def modulated_deformable_conv2d_chw2(input_chw2, offset_chw2, mask, weight_chw2,
     (sh, sw), (ph, pw), (dh, dw) = _pair(stride), _pair(padding), _pair(dilation)
     n, _, h, w, _ = input_chw2.shape
     co, _, kh, kw, _ = weight_chw2.shape
-    ho = (h + 2 * ph - (dh * (kh - 1) + 1)) // sh + 1
-    wo = (w + 2 * pw - (dw * (kw - 1) + 1)) // sw + 1
+    ho, wo = _out_extent(h, kh, sh, ph, dh), _out_extent(w, kw, sw, pw, dw)
     lib = _lib.load()
     ws_bytes = lib.b200_dcn_f16_chw2_workspace_size(n, channels, h, w, co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=input_chw2.device)
     out = torch.empty(n, co, ho, wo, dtype=torch.float16, device=input_chw2.device)
     x, off, msk, wt = (t.contiguous() for t in (input_chw2, offset_chw2, mask.half(), weight_chw2))
     bias_t = bias.half().contiguous() if bias is not None else None
-    with torch.cuda.device(x.device):
-        st = lib.b200_dcn_f16_chw2(x.data_ptr(), wt.data_ptr(), bias_t.data_ptr() if bias_t is not None else None,
-                                   off.data_ptr(), msk.data_ptr(), out.data_ptr(), workspace.data_ptr(), n, channels, h, w,
-                                   co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups, min(n, 32), None,
-                                   _lib.current_stream_ptr())  # fmt: skip
-    _lib.check("b200_dcn_f16_chw2", st)
+    _lib.call("b200_dcn_f16_chw2", x.device, x.data_ptr(), wt.data_ptr(),
+              bias_t.data_ptr() if bias_t is not None else None, off.data_ptr(), msk.data_ptr(), out.data_ptr(),
+              workspace.data_ptr(), n, channels, h, w, co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups,
+              min(n, 32), None)  # fmt: skip
     return out
 
 
@@ -232,8 +223,7 @@ def modulated_deformable_conv2d_int8(input_chw4, scale_i, offset_q, scale_off, m
     co, _, kh, kw, _ = weight_chw4.shape
     if c4 * 4 != channels or weight_chw4.shape[1] * 4 * groups != channels:
         raise ValueError("channels must be a multiple of 4 and match the packed tensors")
-    ho = (h + 2 * ph - (dh * (kh - 1) + 1)) // sh + 1
-    wo = (w + 2 * pw - (dw * (kw - 1) + 1)) // sw + 1
+    ho, wo = _out_extent(h, kh, sh, ph, dh), _out_extent(w, kw, sw, pw, dw)
     if tuple(offset_q.shape) != (n, deform_groups * 2 * kh * kw, ho, wo) or \
             tuple(mask_q.shape) != (n, deform_groups * kh * kw, ho, wo):
         raise ValueError("offset / mask must be [N, deform_groups*2*kh*kw, Ho, Wo] / [N, deform_groups*kh*kw, Ho, Wo]")
@@ -247,12 +237,9 @@ def modulated_deformable_conv2d_int8(input_chw4, scale_i, offset_q, scale_off, m
     bias_t = bias.contiguous() if bias is not None else None
     if bias_t is not None and bias_t.dtype not in (torch.float32, torch.float16):
         raise _lib.B200OpsError("modulated_deformable_conv2d_int8", 1)
-    with torch.cuda.device(x.device):
-        st = lib.b200_dcn_i8(x.data_ptr(), float(scale_i), wt.data_ptr(), float(scale_w),
-                             bias_t.data_ptr() if bias_t is not None else None,
-                             int(bias_t is not None and bias_t.dtype == torch.float16), off.data_ptr(), float(scale_off),
-                             msk.data_ptr(), float(scale_mask), out.data_ptr(), float(scale_o), workspace.data_ptr(), n,
-                             channels, h, w, co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups, min(n, 32), None,
-                             _lib.current_stream_ptr())  # fmt: skip
-    _lib.check("b200_dcn_i8", st)
+    _lib.call("b200_dcn_i8", x.device, x.data_ptr(), float(scale_i), wt.data_ptr(), float(scale_w),
+              bias_t.data_ptr() if bias_t is not None else None,
+              int(bias_t is not None and bias_t.dtype == torch.float16), off.data_ptr(), float(scale_off), msk.data_ptr(),
+              float(scale_mask), out.data_ptr(), float(scale_o), workspace.data_ptr(), n, channels, h, w, co, kw, kh, sw,
+              sh, pw, ph, dw, dh, groups, deform_groups, min(n, 32), None)  # fmt: skip
     return out

@@ -12,8 +12,8 @@ pre-softmax logit gradients), so the attention modules train through the plugin-
 when grad mode is on and an input requires grad, so inference calls run exactly as before. ``…_sca`` with ``accum=``
 given, and INT8, are inference-only.
 """
-import ctypes
 import os
+from typing import NamedTuple
 
 import torch
 from torch.autograd import Function
@@ -103,45 +103,11 @@ def autotune_msda(value, value_spatial_shapes, reference_points, sampling_offset
     if not value.is_cuda or value.dtype not in (torch.float16, torch.float32):
         raise ValueError("autotune_msda: FP16 / FP32 CUDA tensors only (the INT8 op has a single launch shape)")
     args = (value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights)
-    report = {"chosen": "default", "ms": {}, "rejected": []}
-    set_msda_batch_units(1)
-    set_msda_gather_variant(0)
-    try:
-        base = multi_scale_deformable_attn(*args)
-        for _ in range(2 * warmup + 4):  # clocks and caches at their steady state before the first candidate is timed
-            multi_scale_deformable_attn(*args)
-        # the default shape is timed first AND last (its better median counts): a clock ramp or a neighbour's burst
-        # during the sweep must not hand the win to whichever shape happened to run later
-        order = list(MSDA_LAUNCH_SHAPES.items()) + [("default", MSDA_LAUNCH_SHAPES["default"])]
-        for name, (units, strided, variant) in order:
-            if name in report["rejected"]:
-                continue
-            set_msda_batch_units(units, strided)
-            set_msda_gather_variant(variant)
-            out = multi_scale_deformable_attn(*args)
-            if not torch.equal(out, base):
-                report["rejected"].append(name)
-                continue
-            for _ in range(warmup):
-                multi_scale_deformable_attn(*args)
-            evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(iters)]
-            for a, b in evs:
-                a.record()
-                multi_scale_deformable_attn(*args)
-                b.record()
-            torch.cuda.synchronize(value.device)
-            per = sorted(a.elapsed_time(b) for a, b in evs)
-            report["ms"][name] = min(per[len(per) // 2], report["ms"].get(name, float("inf")))
-    finally:
-        set_msda_batch_units(1)
-        set_msda_gather_variant(0)
-    best = min(report["ms"], key=report["ms"].get)
-    if best != "default" and report["ms"][best] < report["ms"]["default"] * (1.0 - min_gain):
-        report["chosen"] = best
-    units, strided, variant = MSDA_LAUNCH_SHAPES[report["chosen"]]
-    set_msda_batch_units(units, strided)
-    set_msda_gather_variant(variant)
-    return report
+    set_msda_launch_shape("default")
+    base = multi_scale_deformable_attn(*args)
+    return _timed_sweep(MSDA_LAUNCH_SHAPES, set_msda_launch_shape, lambda: multi_scale_deformable_attn(*args),
+                        lambda: not torch.equal(multi_scale_deformable_attn(*args), base), iters, warmup, min_gain,
+                        value.device)  # fmt: skip
 
 
 def autotune_msda_fused(run, result, iters=10, warmup=2, tol=1e-4, min_gain=0.02):
@@ -153,21 +119,36 @@ def autotune_msda_fused(run, result, iters=10, warmup=2, tol=1e-4, min_gain=0.02
     bits depend on arrival order in either shape) and it is faster by more than ``min_gain``. Leaves the winner as the
     process-wide gather variant and returns ``{"chosen": "default" | "deep_gather", "ms": {...}, "rejected": [...]}``.
     Local launches only — safe to call per rank before a collective step."""
-    report = {"chosen": "default", "ms": {}, "rejected": []}
-    names = {"default": 0, "deep_gather": 1}
+    variants = {"default": 0, "deep_gather": 1}
     set_msda_gather_variant(0)
-    try:
+    run()
+    base = result().detach().float().clone()
+    scale = max(1.0, float(base.abs().max()))
+
+    def differs():
         run()
-        base = result().detach().float().clone()
-        scale = max(1.0, float(base.abs().max()))
-        for _ in range(2 * warmup + 4):
+        return float((result().detach().float() - base).abs().max()) > tol * scale
+
+    return _timed_sweep(variants, lambda name: set_msda_gather_variant(variants[name]), run, differs, iters, warmup,
+                        min_gain)  # fmt: skip
+
+
+def _timed_sweep(names, apply, run, differs, iters, warmup, min_gain, device=None):
+    """The autotuners' sweep over the launch shapes ``names`` ("default" first), entered with the default applied and
+    its result taken. ``apply(name)`` makes a shape the process-wide setting, ``run()`` launches the op once on the
+    current stream, ``differs()`` launches it once more and tells whether its result disagrees with the default's (such
+    a shape is rejected, whatever its speed). Leaves the chosen shape applied and returns the report."""
+    report = {"chosen": "default", "ms": {}, "rejected": []}
+    try:
+        for _ in range(2 * warmup + 4):  # clocks and caches at their steady state before the first candidate is timed
             run()
-        for name, variant in list(names.items()) + [("default", 0)]:  # default first and last, better median counts
+        # the default shape is timed first AND last (its better median counts): a clock ramp or a neighbour's burst
+        # during the sweep must not hand the win to whichever shape happened to run later
+        for name in [*names, "default"]:
             if name in report["rejected"]:
                 continue
-            set_msda_gather_variant(variant)
-            run()
-            if float((result().detach().float() - base).abs().max()) > tol * scale:
+            apply(name)
+            if differs():
                 report["rejected"].append(name)
                 continue
             for _ in range(warmup):
@@ -177,15 +158,17 @@ def autotune_msda_fused(run, result, iters=10, warmup=2, tol=1e-4, min_gain=0.02
                 a.record()
                 run()
                 b.record()
-            torch.cuda.synchronize()
+            torch.cuda.synchronize(device)
             per = sorted(a.elapsed_time(b) for a, b in evs)
             report["ms"][name] = min(per[len(per) // 2], report["ms"].get(name, float("inf")))
     finally:
-        set_msda_gather_variant(0)
+        apply("default")
     ms = report["ms"]
-    if "deep_gather" in ms and "default" in ms and ms["deep_gather"] < ms["default"] * (1.0 - min_gain):
-        report["chosen"] = "deep_gather"
-    set_msda_gather_variant(names[report["chosen"]])
+    if "default" in ms:
+        best = min(ms, key=ms.get)
+        if best != "default" and ms[best] < ms["default"] * (1.0 - min_gain):
+            report["chosen"] = best
+    apply(report["chosen"])
     return report
 
 
@@ -196,61 +179,64 @@ def set_msda_launch_shape(name: str):
     set_msda_gather_variant(variant)
 
 
-def _v2_workspace(lib, dims, device):
-    """Workspace tensor for the INT8 v2 path, or None when the shape is outside its envelope (or v2 is switched off)."""
-    if not _V2["enabled"]:
-        return None
-    bs, num_keys, num_heads, channels, num_levels, _, num_point, ppg = dims
-    n = lib.b200_msda_i8_workspace_size(bs, num_keys, num_heads, channels, num_levels, num_point, ppg)
-    return torch.empty(n, dtype=torch.uint8, device=device) if n else None
+class _Prepared(NamedTuple):
+    """The tensors an MSDA entry reads — contiguous, int32 level shapes, reference points / offsets / logits in value's
+    dtype (INT8: as given) — and the entry's eight dimension arguments (_lib._MSDA_DIMS)."""
+
+    value: torch.Tensor
+    shapes: torch.Tensor
+    ref: torch.Tensor
+    off: torch.Tensor
+    w: torch.Tensor
+    dims: tuple
+
+    def ptrs(self):
+        return self.value.data_ptr(), self.shapes.data_ptr(), self.ref.data_ptr(), self.off.data_ptr(), self.w.data_ptr()
 
 
-def _launch_int8(lib, dims, value_q, scales, shapes, ref, off, w, out, records=None):
-    """Runs the INT8 plugin op into ``out``: the packed kernel when ``_v2_workspace`` lends a workspace, the round-1
-    kernel otherwise or when the packed one declines the shape (status 1). ``records``: int32 [bs, nq, heads, L*P, 4]
-    for the kernel's own sampling-index records (trace entries), or None."""
-    sv, so, sw, sout = (float(x) for x in scales)
-    half = int(ref.dtype == torch.float16)
-    rec = None if records is None else records.data_ptr()
-    with torch.cuda.device(value_q.device):
-        ws = _v2_workspace(lib, dims, value_q.device)
-        if ws is not None:
-            st = lib.b200_msda_i8_ws(value_q.data_ptr(), sv, shapes.data_ptr(), ref.data_ptr(), half, off.data_ptr(), so,
-                                     w.data_ptr(), sw, *dims, out.data_ptr(), sout, ws.data_ptr(), ws.numel(), rec,
-                                     _lib.current_stream_ptr())  # fmt: skip
-            if st != 1:
-                _lib.check("b200_msda_i8_ws", st)
-                return
-        args = (value_q.data_ptr(), sv, shapes.data_ptr(), ref.data_ptr(), half, off.data_ptr(), so, w.data_ptr(), sw,
-                *dims, out.data_ptr(), sout)  # fmt: skip
-        if records is None:
-            _lib.check("b200_msda_i8", lib.b200_msda_i8(*args, _lib.current_stream_ptr()))
-        else:
-            _lib.check("b200_msda_i8_trace", lib.b200_msda_i8_trace(*args, rec, _lib.current_stream_ptr()))
-
-
-def _check_inputs(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights):
+def _prepare(name, value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, dtype,
+             bev_mask=None):
+    """Checks the inputs of the op ``name`` and makes them what its C entry reads. ``dtype``: value's dtype, FP32 or
+    FP16, which reference points, offsets and logits are cast to; None (INT8) casts nothing. ``bev_mask`` is given by the
+    camera-shared form only: its offsets and logits are ONE copy for all cameras and num_query is read from the mask.
+    Otherwise they are ``bs`` copies and num_query is sampling_offsets.shape[1], the reference plugin's rule."""
     if not value.is_cuda:
-        raise RuntimeError("multi_scale_deformable_attn: value must be a CUDA tensor (no CPU fallback exists)")
+        raise RuntimeError(f"{name}: value must be a CUDA tensor (no CPU fallback exists)")
     if value.dim() != 4:
         raise ValueError("value must be [bs, num_keys, num_heads, channels]")
     bs, num_keys, num_heads, channels = value.shape
     num_levels = value_spatial_shapes.shape[0]
-    num_query = sampling_offsets.shape[1]
     if reference_points.shape[-1] % 2 != 0:
         raise ValueError("reference_points last dim must hold (x, y) pairs")
     points_per_group = reference_points.shape[-1] // 2
     all_points = attention_weights.shape[-1]
     if all_points % num_levels != 0:
         raise ValueError("attention_weights last dim must be num_levels * num_points")
-    num_point = all_points // num_levels
-    if sampling_offsets.numel() != bs * num_query * num_heads * all_points * 2:
-        raise ValueError("sampling_offsets does not match [bs, num_query, num_heads, num_levels*num_points*2]")
-    if attention_weights.numel() != bs * num_query * num_heads * all_points:
-        raise ValueError("attention_weights does not match [bs, num_query, num_heads, num_levels*num_points]")
+    if bev_mask is None:
+        num_query, copies, lead = sampling_offsets.shape[1], bs, "bs"
+    else:
+        num_query, copies, lead = bev_mask.numel() // bs, 1, "1"
+    if sampling_offsets.numel() != copies * num_query * num_heads * all_points * 2:
+        raise ValueError(f"sampling_offsets does not match [{lead}, num_query, num_heads, num_levels*num_points*2]")
+    if attention_weights.numel() != copies * num_query * num_heads * all_points:
+        raise ValueError(f"attention_weights does not match [{lead}, num_query, num_heads, num_levels*num_points]")
     if reference_points.numel() != bs * num_query * points_per_group * 2:
         raise ValueError("reference_points does not match [bs, num_query, 1, 2*points_per_group]")
-    return bs, num_keys, num_heads, channels, num_levels, num_query, num_point, points_per_group
+    if dtype is not None:
+        if dtype not in (torch.float32, torch.float16):
+            raise _lib.B200OpsError(name, 1)
+        reference_points = _cast(reference_points, dtype)
+        sampling_offsets = _cast(sampling_offsets, dtype)
+        attention_weights = _cast(attention_weights, dtype)
+    dims = (bs, num_keys, num_heads, channels, num_levels, num_query, all_points // num_levels, points_per_group)
+    return _Prepared(value.contiguous(), _shapes_i32(value_spatial_shapes, value.device), reference_points.contiguous(),
+                     sampling_offsets.contiguous(), attention_weights.contiguous(), dims)  # fmt: skip
+
+
+def _cast(t, dtype):
+    """``t.to(dtype)``, which returns ``t`` itself when the dtype already matches but still costs about a microsecond of
+    host time to find that out."""
+    return t if t.dtype == dtype else t.to(dtype)
 
 
 def _shapes_i32(value_spatial_shapes, device):
@@ -258,21 +244,48 @@ def _shapes_i32(value_spatial_shapes, device):
     return value_spatial_shapes.to(device=device, dtype=torch.int32).contiguous()
 
 
-def _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, use_h2, out=None,
-                  keep=None):
-    """``keep``: a list that receives the tensors the kernel actually read (contiguous, in value's dtype) and the
-    dimension tuple, for the backward."""
-    dims = _check_inputs(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights)
-    bs, _, num_heads, channels, _, num_query, _, _ = dims
-    lib = _lib.load()
+def _per_camera(p):
+    """The camera-shared form's inputs with offsets and logits repeated for the ``bs`` cameras, as the plugin op reads
+    them."""
+    bs, _, num_heads, _, num_levels, num_query, num_point, _ = p.dims
+    n = num_levels * num_point
+    return p._replace(off=p.off.reshape(1, num_query, num_heads, n * 2).expand(bs, -1, -1, -1).contiguous(),
+                      w=p.w.reshape(1, num_query, num_heads, n).expand(bs, -1, -1, -1).contiguous())
+
+
+def _v2_workspace(dims, device):
+    """Workspace tensor for the INT8 v2 path, or None when the shape is outside its envelope (or v2 is switched off)."""
+    if not _V2["enabled"]:
+        return None
+    bs, num_keys, num_heads, channels, num_levels, _, num_point, ppg = dims
+    n = _lib.load().b200_msda_i8_workspace_size(bs, num_keys, num_heads, channels, num_levels, num_point, ppg)
+    return torch.empty(n, dtype=torch.uint8, device=device) if n else None
+
+
+def _launch_int8(p, scales, out, records=None):
+    """Runs the INT8 plugin op on the prepared inputs ``p`` into ``out``: the packed kernel when ``_v2_workspace`` lends
+    a workspace, the round-1 kernel otherwise or when the packed one declines the shape (status 1). ``records``: int32
+    [bs, nq, heads, L*P, 4] for the kernel's own sampling-index records (trace entries), or None."""
+    sv, so, sw, sout = (float(x) for x in scales)
+    dev = p.value.device
+    rec = None if records is None else records.data_ptr()
+    args = (p.value.data_ptr(), sv, p.shapes.data_ptr(), p.ref.data_ptr(), int(p.ref.dtype == torch.float16),
+            p.off.data_ptr(), so, p.w.data_ptr(), sw, *p.dims, out.data_ptr(), sout)  # fmt: skip
+    ws = _v2_workspace(p.dims, dev)
+    if ws is not None and _lib.call("b200_msda_i8_ws", dev, *args, ws.data_ptr(), ws.numel(), rec, accept=(0, 1)) == 0:
+        return
+    if records is None:
+        _lib.call("b200_msda_i8", dev, *args)
+    else:
+        _lib.call("b200_msda_i8_trace", dev, *args, rec)
+
+
+def _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, use_h2, out=None):
+    """The FP32 / FP16 plugin op. Returns its output and the prepared inputs the kernel read (for the backward)."""
     dt = value.dtype
-    if dt not in (torch.float32, torch.float16):
-        raise _lib.B200OpsError("multi_scale_deformable_attn", 1)
-    value = value.contiguous()
-    shapes = _shapes_i32(value_spatial_shapes, value.device)
-    ref = reference_points.to(dt).contiguous()
-    off = sampling_offsets.to(dt).contiguous()
-    w = attention_weights.to(dt).contiguous()
+    p = _prepare("multi_scale_deformable_attn", value, value_spatial_shapes, reference_points, sampling_offsets,
+                 attention_weights, dt)  # fmt: skip
+    bs, _, num_heads, channels, _, num_query, _, _ = p.dims
     if out is None:
         out = torch.empty(bs, num_query, num_heads, channels, dtype=dt, device=value.device)
     elif out.dtype != dt or not out.is_contiguous() or out.numel() != bs * num_query * num_heads * channels:
@@ -281,46 +294,47 @@ def _msda_forward(value, value_spatial_shapes, reference_points, sampling_offset
         name = "b200_msda_f32"
     else:
         name = "b200_msda_f16_h2" if use_h2 and channels % 2 == 0 else "b200_msda_f16"
-    with torch.cuda.device(value.device):
-        st = getattr(lib, name)(value.data_ptr(), shapes.data_ptr(), ref.data_ptr(), off.data_ptr(), w.data_ptr(),
-                                *dims, out.data_ptr(), _lib.current_stream_ptr())  # fmt: skip
-    _lib.check(name, st)
-    if keep is not None:
-        keep.extend((value, shapes, ref, off, w, dims))
-    return out
+    _lib.call(name, value.device, *p.ptrs(), *p.dims, out.data_ptr())
+    return out, p
+
+
+def _save(ctx, p, inputs, *extra):
+    """Keeps for the backward the tensors the forward's kernel read (and ``extra``), its dimensions, and the dtype and
+    shape of the differentiable ``inputs`` (value, reference points, offsets, logits), which their gradients take."""
+    ctx.save_for_backward(p.value, p.shapes, p.ref, p.off, p.w, *extra)
+    ctx.dims = p.dims
+    ctx.like = [(t.dtype, t.shape) for t in inputs]
+
+
+def _backward_launch(prefix, p, args, needs, accept=(0,)):
+    """Runs the backward entry ``{prefix}_backward_{f32|f16}`` — b200_msda_, b200_msda_sca_ or b200_msda_sca_shared_ —
+    on the forward's inputs ``p``. ``args``: the tensors the entry takes between the logits and the gradients (grad_out;
+    bev_mask and grad_slots for the fused forms). ``needs``: the op's ``needs_input_grad``, which selects the value,
+    reference-point, offset and logit gradients to compute. Returns them (None where not wanted), or None when the entry
+    declined with a non-zero status in ``accept``."""
+    dt, dev = p.value.dtype, p.value.device
+    ws_bytes = _lib.load().b200_msda_backward_workspace_size(int(dt == torch.float16), *p.dims)
+    if ws_bytes == 0:
+        raise _lib.B200OpsError("b200_msda_backward_workspace_size", 2)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    grads = [torch.empty_like(t) if needs[i] else None for i, t in ((0, p.value), (2, p.ref), (3, p.off), (4, p.w))]
+    name = f"{prefix}_backward_{'f32' if dt == torch.float32 else 'f16'}"
+    st = _lib.call(name, dev, *p.ptrs(), *[t.data_ptr() for t in args],
+                   *[g.data_ptr() if g is not None else None for g in grads], ws.data_ptr(), *p.dims, accept=accept)
+    return None if st else grads
+
+
+def _grads_like(ctx, grads):
+    """The op's gradients: value, reference points, offsets and logits in their inputs' dtypes and shapes."""
+    gv, gr, go, gw = (_cast(g, d).reshape(shp) if g is not None else None for g, (d, shp) in zip(grads, ctx.like))
+    return gv, None, gr, go, gw
 
 
 def _msda_autograd_forward(ctx, value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, use_h2):
-    if not any(ctx.needs_input_grad):
-        return _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, use_h2)
-    keep = []
-    out = _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, use_h2,
-                        keep=keep)
-    ctx.save_for_backward(*keep[:5])
-    ctx.dims = keep[5]
-    ctx.like = [(t.dtype, t.shape) for t in (value, reference_points, sampling_offsets, attention_weights)]
+    out, p = _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, use_h2)
+    if any(ctx.needs_input_grad):
+        _save(ctx, p, (value, reference_points, sampling_offsets, attention_weights))
     return out
-
-
-def _msda_backward(ctx, grad_out):
-    value, shapes, ref, off, w = ctx.saved_tensors
-    dims, dt = ctx.dims, value.dtype
-    lib = _lib.load()
-    go = grad_out.to(dt).contiguous()
-    want = (ctx.needs_input_grad[0], ctx.needs_input_grad[2], ctx.needs_input_grad[3], ctx.needs_input_grad[4])
-    grads = [torch.empty_like(t) if n else None for t, n in zip((value, ref, off, w), want)]
-    ws_bytes = lib.b200_msda_backward_workspace_size(int(dt == torch.float16), *dims)
-    if ws_bytes == 0:
-        raise _lib.B200OpsError("b200_msda_backward_workspace_size", 2)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=value.device)
-    name = "b200_msda_backward_f32" if dt == torch.float32 else "b200_msda_backward_f16"
-    with torch.cuda.device(value.device):
-        st = getattr(lib, name)(value.data_ptr(), shapes.data_ptr(), ref.data_ptr(), off.data_ptr(), w.data_ptr(),
-                                go.data_ptr(), *(g.data_ptr() if g is not None else None for g in grads),
-                                ws.data_ptr(), *dims, _lib.current_stream_ptr())  # fmt: skip
-    _lib.check(name, st)
-    gv, gr, gs, gw = (g.to(d).reshape(shp) if g is not None else None for g, (d, shp) in zip(grads, ctx.like))
-    return gv, None, gr, gs, gw
 
 
 class _MultiScaleDeformableAttnFunction(Function):
@@ -345,7 +359,9 @@ class _MultiScaleDeformableAttnFunction(Function):
         """(grad_value, None, grad_reference_points, grad_sampling_offsets, grad_attention_weights), each in its input's
         dtype and shape; ``None`` for inputs that do not require a gradient. The offset, logit and reference-point
         gradients are bit-reproducible; grad_value is summed with float atomics."""
-        return _msda_backward(ctx, grad_out)
+        p = _Prepared(*ctx.saved_tensors, ctx.dims)
+        go = _cast(grad_out, p.value.dtype).contiguous()
+        return _grads_like(ctx, _backward_launch("b200_msda", p, (go,), ctx.needs_input_grad))
 
 
 class _MultiScaleDeformableAttnFunction2(_MultiScaleDeformableAttnFunction):
@@ -364,7 +380,8 @@ def multi_scale_deformable_attn_out(value, value_spatial_shapes, reference_point
                                     out):
     """The plugin op writing into a caller-owned ``out`` (no allocation on the call path; used by HostMSDA, whose
     device slots are fixed so that the stream-ordered allocator never has to synchronise)."""
-    return _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, False, out)
+    return _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, False,
+                         out)[0]  # fmt: skip
 
 
 _multi_scale_deformable_attn_gpu = _MultiScaleDeformableAttnFunction.apply
@@ -392,18 +409,13 @@ def multi_scale_deformable_attn_int8(value_q, scale_value, value_spatial_shapes,
     int8 entry (TensorRT supplies the scales through PluginTensorDesc); this mirrors the C launcher's argument list
     (…Kernel.h:29-38)."""
     assert value_q.is_cuda and value_q.dtype == torch.int8
-    dims = _check_inputs(value_q, value_spatial_shapes, reference_points, offsets_q, weights_q)
-    bs, _, num_heads, channels, _, num_query, _, _ = dims
+    p = _prepare("multi_scale_deformable_attn_int8", value_q, value_spatial_shapes, reference_points, offsets_q,
+                 weights_q, None)  # fmt: skip
     if reference_points.dtype not in (torch.float16, torch.float32):
         raise _lib.B200OpsError("multi_scale_deformable_attn_int8", 1)
-    lib = _lib.load()
-    value_q = value_q.contiguous()
-    shapes = _shapes_i32(value_spatial_shapes, value_q.device)
-    ref = reference_points.contiguous()
-    off = offsets_q.contiguous()
-    w = weights_q.contiguous()
+    bs, _, num_heads, channels, _, num_query, _, _ = p.dims
     out = torch.empty(bs, num_query, num_heads, channels, dtype=torch.int8, device=value_q.device)
-    _launch_int8(lib, dims, value_q, (scale_value, scale_offset, scale_weight, scale_out), shapes, ref, off, w, out)
+    _launch_int8(p, (scale_value, scale_offset, scale_weight, scale_out), out)
     return out
 
 
@@ -418,83 +430,74 @@ def _wants_grad(tensors, bev_mask, name):
     return any(isinstance(t, torch.Tensor) and t.requires_grad for t in tensors)
 
 
-def _sca_backward(ctx, grad_slots, shared):
-    """Gradients of the fused SCA forms: the fused backward kernel when the forward ran the fused kernel, otherwise
-    (the forward took the plugin-op fallback) the plugin-op backward fed ``go = bev_mask * grad_slots`` per camera,
-    summed over the cameras for the shared offsets and logits."""
-    value, shapes, ref, off, w, mask = ctx.saved_tensors
-    dims, dt = ctx.dims, value.dtype
-    bs, _, num_heads, channels, _, num_query, _, _ = dims
-    lib = _lib.load()
-    gs = grad_slots.to(torch.float32).contiguous()
-    if gs.data_ptr() % 16:
-        gs = gs.clone()  # a fresh allocation is 16-byte aligned, as the fused kernel needs
-    want = (ctx.needs_input_grad[0], ctx.needs_input_grad[2], ctx.needs_input_grad[3], ctx.needs_input_grad[4])
-    ws_bytes = lib.b200_msda_backward_workspace_size(int(dt == torch.float16), *dims)
-    if ws_bytes == 0:
-        raise _lib.B200OpsError("b200_msda_backward_workspace_size", 2)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=value.device)
-    sfx = "f32" if dt == torch.float32 else "f16"
-    st = 1
-    if ctx.fused:
-        grads = [torch.empty_like(t) if n else None for t, n in zip((value, ref, off, w), want)]
-        name = f"b200_msda_sca{'_shared' if shared else ''}_backward_{sfx}"
-        with torch.cuda.device(value.device):
-            st = getattr(lib, name)(value.data_ptr(), shapes.data_ptr(), ref.data_ptr(), off.data_ptr(), w.data_ptr(),
-                                    mask.data_ptr(), gs.data_ptr(), *(g.data_ptr() if g is not None else None for g in grads),
-                                    ws.data_ptr(), *dims, _lib.current_stream_ptr())  # fmt: skip
-        if st != 1:
-            _lib.check(name, st)
-    if st == 1:
-        go = (mask.unsqueeze(-1) * gs).to(dt).reshape(bs, num_query, num_heads, channels)
+def _sca_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, bev_mask, accum,
+                 shared):
+    """Both fused SCA forms: ``…_sca`` (``shared`` False; adds into ``accum``, allocated when None) and
+    ``…_sca_shared``. Returns the result, the prepared inputs, the fp32 mask and whether the fused kernel ran (False:
+    the plugin-op fallback)."""
+    form = "sca_shared" if shared else "sca"
+    dt = value.dtype
+    p = _prepare(f"multi_scale_deformable_attn_{form}", value, value_spatial_shapes, reference_points, sampling_offsets,
+                 attention_weights, dt, bev_mask if shared else None)  # fmt: skip
+    bs, _, num_heads, channels, _, num_query, _, _ = p.dims
+    mask = _cast(bev_mask.reshape(bs, num_query), torch.float32).contiguous()
+    if shared:
+        res = torch.empty(num_query, num_heads * channels, dtype=torch.float32, device=value.device)
+    elif accum is None:
+        res = torch.zeros(num_query, num_heads * channels, dtype=torch.float32, device=value.device)
+    elif accum.dtype != torch.float32 or not accum.is_contiguous() or accum.numel() != num_query * num_heads * channels:
+        raise ValueError("accum must be a contiguous float32 [num_query, heads*channels] tensor")
+    else:
+        res = accum
+    name = f"b200_msda_{form}_{'f32' if dt == torch.float32 else 'f16'}"
+    fused = _lib.call(name, value.device, *p.ptrs(), mask.data_ptr(), *p.dims, res.data_ptr(), accept=(0, 1)) == 0
+    if not fused:
+        # shapes the fused kernel does not take (e.g. channels != 32, more than 64 points, unaligned tensors): the plugin
+        # op on bs copies of offsets / logits, then the masked camera sum
+        q = _per_camera(p) if shared else p
+        out, _ = _msda_forward(q.value, q.shapes, q.ref, q.off, q.w, False)
+        total = (out.reshape(bs, num_query, -1).float() * mask.unsqueeze(-1)).sum(0)
         if shared:
-            off = off.reshape(1, num_query, num_heads, -1).expand(bs, -1, -1, -1).contiguous()
-            w = w.reshape(1, num_query, num_heads, -1).expand(bs, -1, -1, -1).contiguous()
-        grads = [torch.empty_like(t) if n else None for t, n in zip((value, ref, off, w), want)]
-        name = f"b200_msda_backward_{sfx}"
-        with torch.cuda.device(value.device):
-            st = getattr(lib, name)(value.data_ptr(), shapes.data_ptr(), ref.data_ptr(), off.data_ptr(), w.data_ptr(),
-                                    go.data_ptr(), *(g.data_ptr() if g is not None else None for g in grads),
-                                    ws.data_ptr(), *dims, _lib.current_stream_ptr())  # fmt: skip
-        _lib.check(name, st)
-        if shared:
-            grads[2:] = [g.float().sum(0) if g is not None else None for g in grads[2:]]
-    gv, gr, go_, gw = (g.to(d).reshape(shp) if g is not None else None for g, (d, shp) in zip(grads, ctx.like))
-    return gv, None, gr, go_, gw, None
+            res = total
+        else:
+            res += total
+    return res, p, mask, fused
 
 
 class _MsdaScaFunction(Function):
+    """Autograd of the fused SCA forms; ``shared`` selects the camera-shared one."""
+
     @staticmethod
-    def forward(ctx, value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, bev_mask):
-        keep = []
-        out = _msda_sca_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights,
-                                bev_mask, None, keep)  # fmt: skip
-        ctx.save_for_backward(*keep[:6])
-        ctx.dims, ctx.fused = keep[6], keep[7]
-        ctx.like = [(t.dtype, t.shape) for t in (value, reference_points, sampling_offsets, attention_weights)]
+    def forward(ctx, value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, bev_mask,
+                shared):  # fmt: skip
+        out, p, mask, ctx.fused = _sca_forward(value, value_spatial_shapes, reference_points, sampling_offsets,
+                                               attention_weights, bev_mask, None, shared)  # fmt: skip
+        ctx.shared = shared
+        _save(ctx, p, (value, reference_points, sampling_offsets, attention_weights), mask)
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, grad_slots):
-        return _sca_backward(ctx, grad_slots, False)
-
-
-class _MsdaScaSharedFunction(Function):
-    @staticmethod
-    def forward(ctx, value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, bev_mask):
-        keep = []
-        out = _msda_sca_shared_forward(value, value_spatial_shapes, reference_points, sampling_offsets,
-                                       attention_weights, bev_mask, keep)  # fmt: skip
-        ctx.save_for_backward(*keep[:6])
-        ctx.dims, ctx.fused = keep[6], keep[7]
-        ctx.like = [(t.dtype, t.shape) for t in (value, reference_points, sampling_offsets, attention_weights)]
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_slots):
-        return _sca_backward(ctx, grad_slots, True)
+        """The fused backward kernel when the forward ran the fused kernel; otherwise (the forward took the plugin-op
+        fallback, or the backward kernel declines the shape) the plugin-op backward fed ``go = bev_mask * grad_slots``
+        per camera, summed over the cameras for the shared offsets and logits."""
+        *saved, mask = ctx.saved_tensors
+        p = _Prepared(*saved, ctx.dims)
+        bs, _, num_heads, channels, _, num_query, _, _ = p.dims
+        gs = _cast(grad_slots, torch.float32).contiguous()
+        if gs.data_ptr() % 16:
+            gs = gs.clone()  # a fresh allocation is 16-byte aligned, as the fused kernel needs
+        grads = None
+        if ctx.fused:
+            prefix = "b200_msda_sca_shared" if ctx.shared else "b200_msda_sca"
+            grads = _backward_launch(prefix, p, (mask, gs), ctx.needs_input_grad, accept=(0, 1))
+        if grads is None:
+            go = _cast(mask.unsqueeze(-1) * gs, p.value.dtype).reshape(bs, num_query, num_heads, channels)
+            grads = _backward_launch("b200_msda", _per_camera(p) if ctx.shared else p, (go,), ctx.needs_input_grad)
+            if ctx.shared:
+                grads[2:] = [g.float().sum(0) if g is not None else None for g in grads[2:]]
+        return (*_grads_like(ctx, grads), None, None)
 
 
 def multi_scale_deformable_attn_sca(value, value_spatial_shapes, reference_points, sampling_offsets,
@@ -512,45 +515,9 @@ def multi_scale_deformable_attn_sca(value, value_spatial_shapes, reference_point
     if accum is None and _wants_grad((value, reference_points, sampling_offsets, attention_weights), bev_mask,
                                      "multi_scale_deformable_attn_sca"):  # fmt: skip
         return _MsdaScaFunction.apply(value, value_spatial_shapes, reference_points, sampling_offsets,
-                                      attention_weights, bev_mask)  # fmt: skip
-    return _msda_sca_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights,
-                             bev_mask, accum)  # fmt: skip
-
-
-def _msda_sca_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, bev_mask,
-                      accum, keep=None):
-    """``keep``: a list that receives the tensors the kernel read, the dimension tuple and whether the fused kernel ran
-    (False: the plugin-op fallback), for the backward."""
-    dims = _check_inputs(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights)
-    bs, _, num_heads, channels, _, num_query, _, _ = dims
-    dt = value.dtype
-    if dt not in (torch.float32, torch.float16):
-        raise _lib.B200OpsError("multi_scale_deformable_attn_sca", 1)
-    lib = _lib.load()
-    value = value.contiguous()
-    shapes = _shapes_i32(value_spatial_shapes, value.device)
-    ref = reference_points.to(dt).contiguous()
-    off = sampling_offsets.to(dt).contiguous()
-    w = attention_weights.to(dt).contiguous()
-    mask = bev_mask.reshape(bs, num_query).to(torch.float32).contiguous()
-    if accum is None:
-        accum = torch.zeros(num_query, num_heads * channels, dtype=torch.float32, device=value.device)
-    else:
-        if accum.dtype != torch.float32 or not accum.is_contiguous() or accum.numel() != num_query * num_heads * channels:
-            raise ValueError("accum must be a contiguous float32 [num_query, heads*channels] tensor")
-    name = "b200_msda_sca_f32" if dt == torch.float32 else "b200_msda_sca_f16"
-    with torch.cuda.device(value.device):
-        st = getattr(lib, name)(value.data_ptr(), shapes.data_ptr(), ref.data_ptr(), off.data_ptr(), w.data_ptr(),
-                                mask.data_ptr(), *dims, accum.data_ptr(), _lib.current_stream_ptr())  # fmt: skip
-        if keep is not None:
-            keep.extend((value, shapes, ref, off, w, mask, dims, st != 1))
-        if st == 1:
-            # shapes neither fused kernel takes (channels != 32, more than 64 points): plugin op + masked camera sum
-            out = _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, False)
-            accum += (out.reshape(bs, num_query, -1).float() * mask.unsqueeze(-1)).sum(0)
-            return accum
-    _lib.check(name, st)
-    return accum
+                                      attention_weights, bev_mask, False)  # fmt: skip
+    return _sca_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, bev_mask,
+                        accum, False)[0]  # fmt: skip
 
 
 def multi_scale_deformable_attn_queue_mean(value, value_spatial_shapes, reference_points, sampling_offsets,
@@ -587,60 +554,10 @@ def multi_scale_deformable_attn_sca_shared(value, value_spatial_shapes, referenc
     a query no camera sees gets zeros there."""
     if _wants_grad((value, reference_points, sampling_offsets, attention_weights), bev_mask,
                    "multi_scale_deformable_attn_sca_shared"):  # fmt: skip
-        return _MsdaScaSharedFunction.apply(value, value_spatial_shapes, reference_points, sampling_offsets,
-                                            attention_weights, bev_mask)  # fmt: skip
-    return _msda_sca_shared_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights,
-                                    bev_mask)  # fmt: skip
-
-
-def _msda_sca_shared_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights,
-                             bev_mask, keep=None):
-    """``keep``: as for ``_msda_sca_forward``."""
-    if not value.is_cuda:
-        raise RuntimeError("multi_scale_deformable_attn_sca_shared: value must be a CUDA tensor (no CPU fallback exists)")
-    if value.dim() != 4:
-        raise ValueError("value must be [bs, num_keys, num_heads, channels]")
-    bs, num_keys, num_heads, channels = value.shape
-    dt = value.dtype
-    if dt not in (torch.float32, torch.float16):
-        raise _lib.B200OpsError("multi_scale_deformable_attn_sca_shared", 1)
-    num_levels = value_spatial_shapes.shape[0]
-    all_points = attention_weights.shape[-1]
-    if all_points % num_levels != 0:
-        raise ValueError("attention_weights last dim must be num_levels * num_points")
-    num_query = bev_mask.numel() // bs
-    points_per_group = reference_points.shape[-1] // 2
-    if sampling_offsets.numel() != num_query * num_heads * all_points * 2:
-        raise ValueError("sampling_offsets must be ONE copy: [num_query, num_heads, num_levels*num_points*2]")
-    if attention_weights.numel() != num_query * num_heads * all_points:
-        raise ValueError("attention_weights must be ONE copy: [num_query, num_heads, num_levels*num_points]")
-    if reference_points.numel() != bs * num_query * points_per_group * 2:
-        raise ValueError("reference_points does not match [bs, num_query, 1, 2*points_per_group]")
-    lib = _lib.load()
-    value = value.contiguous()
-    shapes = _shapes_i32(value_spatial_shapes, value.device)
-    ref = reference_points.to(dt).contiguous()
-    off = sampling_offsets.to(dt).contiguous()
-    w = attention_weights.to(dt).contiguous()
-    mask = bev_mask.reshape(bs, num_query).to(torch.float32).contiguous()
-    slots = torch.empty(num_query, num_heads * channels, dtype=torch.float32, device=value.device)
-    name = "b200_msda_sca_shared_f32" if dt == torch.float32 else "b200_msda_sca_shared_f16"
-    with torch.cuda.device(value.device):
-        st = getattr(lib, name)(value.data_ptr(), shapes.data_ptr(), ref.data_ptr(), off.data_ptr(), w.data_ptr(),
-                                mask.data_ptr(), bs, num_keys, num_heads, channels, num_levels, num_query,
-                                all_points // num_levels, points_per_group, slots.data_ptr(),
-                                _lib.current_stream_ptr())  # fmt: skip
-        if keep is not None:
-            dims = (bs, num_keys, num_heads, channels, num_levels, num_query, all_points // num_levels, points_per_group)
-            keep.extend((value, shapes, ref, off, w, mask, dims, st != 1))
-        if st == 1:
-            # shapes the fused kernel does not take: plugin op on bs copies of offsets / logits + masked camera sum
-            rep_off = off.reshape(1, num_query, num_heads, all_points * 2).expand(bs, -1, -1, -1)
-            rep_w = w.reshape(1, num_query, num_heads, all_points).expand(bs, -1, -1, -1)
-            out = _msda_forward(value, shapes, ref, rep_off, rep_w, False)
-            return (out.reshape(bs, num_query, -1).float() * mask.unsqueeze(-1)).sum(0)
-    _lib.check(name, st)
-    return slots
+        return _MsdaScaFunction.apply(value, value_spatial_shapes, reference_points, sampling_offsets,
+                                      attention_weights, bev_mask, True)  # fmt: skip
+    return _sca_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, bev_mask,
+                        None, True)[0]  # fmt: skip
 
 
 def msda_sampling_indices(value_spatial_shapes, reference_points, sampling_offsets, num_heads):
@@ -654,11 +571,8 @@ def msda_sampling_indices(value_spatial_shapes, reference_points, sampling_offse
     ref = reference_points.contiguous()
     off = sampling_offsets.to(ref.dtype).contiguous()
     rec = torch.empty(bs, nq, num_heads, NP, 4, dtype=torch.int32, device=ref.device)
-    with torch.cuda.device(ref.device):
-        st = _lib.load().b200_msda_debug_indices(int(ref.dtype == torch.float16), shapes.data_ptr(), ref.data_ptr(),
-                                                 off.data_ptr(), bs, num_heads, L, nq, NP // L, G, rec.data_ptr(),
-                                                 _lib.current_stream_ptr())  # fmt: skip
-    _lib.check("b200_msda_debug_indices", st)
+    _lib.call("b200_msda_debug_indices", ref.device, int(ref.dtype == torch.float16), shapes.data_ptr(), ref.data_ptr(),
+              off.data_ptr(), bs, num_heads, L, nq, NP // L, G, rec.data_ptr())  # fmt: skip
     return rec
 
 
@@ -668,24 +582,15 @@ def msda_trace(value, value_spatial_shapes, reference_points, sampling_offsets, 
     while it samples (C entries b200_msda_{f32,f16,i8}_trace). ``scales`` = (scale_value, scale_offset, scale_weight,
     scale_out) selects the INT8 kernel (int8 value / offsets / logits, float or half reference points)."""
     assert value.is_cuda
-    dims = _check_inputs(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights)
-    bs, _, num_heads, channels, num_levels, num_query, num_point, _ = dims
-    lib = _lib.load()
     dt = value.dtype
-    value = value.contiguous()
-    shapes = _shapes_i32(value_spatial_shapes, value.device)
+    p = _prepare("msda_trace", value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights,
+                 None if dt == torch.int8 else dt)  # fmt: skip
+    bs, _, num_heads, channels, num_levels, num_query, num_point, _ = p.dims
     out = torch.empty(bs, num_query, num_heads, channels, dtype=dt, device=value.device)
     rec = torch.empty(bs, num_query, num_heads, num_levels * num_point, 4, dtype=torch.int32, device=value.device)
     if dt == torch.int8:
-        ref, off, w = reference_points.contiguous(), sampling_offsets.contiguous(), attention_weights.contiguous()
-        _launch_int8(lib, dims, value, scales, shapes, ref, off, w, out, rec)
-    elif dt in (torch.float32, torch.float16):
-        ref, off, w = (t.to(dt).contiguous() for t in (reference_points, sampling_offsets, attention_weights))
-        name = "b200_msda_f32_trace" if dt == torch.float32 else "b200_msda_f16_trace"
-        with torch.cuda.device(value.device):
-            st = getattr(lib, name)(value.data_ptr(), shapes.data_ptr(), ref.data_ptr(), off.data_ptr(), w.data_ptr(),
-                                    *dims, out.data_ptr(), rec.data_ptr(), _lib.current_stream_ptr())  # fmt: skip
-        _lib.check(name, st)
+        _launch_int8(p, scales, out, rec)
     else:
-        raise _lib.B200OpsError("msda_trace", 1)
+        name = "b200_msda_f32_trace" if dt == torch.float32 else "b200_msda_f16_trace"
+        _lib.call(name, value.device, *p.ptrs(), *p.dims, out.data_ptr(), rec.data_ptr())
     return out, rec

@@ -37,12 +37,9 @@ def _launch(ref3d, pc_range, lidar2img, image_shape, bev_h, bev_w, D, dtype, dev
     ref_cam = torch.empty(cams, 1, Q, D, 2, dtype=dtype, device=device)
     bev_mask = torch.empty(cams, Q, 1, dtype=dtype, device=device)
     pcr = (ctypes.c_double * 6)(*[float(v) for v in pc_range])
-    with torch.cuda.device(device):
-        st = _lib.load().b200_bev_point_sampling(ref3d.data_ptr() if ref3d is not None else None, pcr,
-                                                 lidar2img.data_ptr(), cams, int(image_shape[0]), int(image_shape[1]),
-                                                 bev_h, bev_w, D, int(dtype == torch.float16), ref_cam.data_ptr(),
-                                                 bev_mask.data_ptr(), _lib.current_stream_ptr())  # fmt: skip
-    _lib.check("b200_bev_point_sampling", st)
+    _lib.call("b200_bev_point_sampling", device, ref3d.data_ptr() if ref3d is not None else None, pcr,
+              lidar2img.data_ptr(), cams, int(image_shape[0]), int(image_shape[1]), bev_h, bev_w, D,
+              int(dtype == torch.float16), ref_cam.data_ptr(), bev_mask.data_ptr())  # fmt: skip
     return ref_cam, bev_mask
 
 

@@ -33,12 +33,6 @@ def _scalars(img, angle, center, dtype):
     return angle.contiguous(), center.contiguous()
 
 
-def _call(name, img, *args):
-    with torch.cuda.device(img.device):
-        st = getattr(_lib.load(), name)(*args, _lib.current_stream_ptr())
-    _lib.check(name, st)
-
-
 def _is_hwc_view(img):
     """True for a [C, H, W] view whose memory is a dense [H, W, C] tensor (what .view(H, W, C).permute(2, 0, 1) gives)."""
     c, h, w = img.shape
@@ -60,8 +54,8 @@ def _forward(img, angle, center, interpolation):
     angle, center = _scalars(img, angle, center, img.dtype)
     out = torch.empty_like(img)
     name = "b200_rotate_f32" if img.dtype == torch.float32 else "b200_rotate_f16"
-    _call(name, img, out.data_ptr(), img.data_ptr(), angle.data_ptr(), center.data_ptr(), (ctypes.c_int * 3)(c, h, w),
-          int(interpolation))  # fmt: skip
+    _lib.call(name, img.device, out.data_ptr(), img.data_ptr(), angle.data_ptr(), center.data_ptr(),
+              (ctypes.c_int * 3)(c, h, w), int(interpolation))  # fmt: skip
     return out
 
 
@@ -109,8 +103,8 @@ def rotate_hwc(img_hwc, angle, center, interpolation="nearest"):
     angle, center = _scalars(img_hwc, angle, center, img_hwc.dtype)
     out = torch.empty_like(img_hwc)
     mode = _MODE[interpolation] if isinstance(interpolation, str) else int(interpolation)
-    _call("b200_rotate_hwc", img_hwc, out.data_ptr(), img_hwc.data_ptr(), angle.data_ptr(), center.data_ptr(),
-          0 if img_hwc.dtype == torch.float32 else 1, (ctypes.c_int * 3)(c, h, w), mode)  # fmt: skip
+    _lib.call("b200_rotate_hwc", img_hwc.device, out.data_ptr(), img_hwc.data_ptr(), angle.data_ptr(),
+              center.data_ptr(), 0 if img_hwc.dtype == torch.float32 else 1, (ctypes.c_int * 3)(c, h, w), mode)  # fmt: skip
     return out
 
 
@@ -121,8 +115,8 @@ def rotate_chw2(img_chw2, channels, angle, center, interpolation="nearest"):
     _, h, w, _ = img_chw2.shape
     angle, center = _scalars(img_chw2, angle, center, torch.float16)
     out = torch.empty_like(img_chw2)
-    _call("b200_rotate_f16_h2", img_chw2, out.data_ptr(), img_chw2.data_ptr(), angle.data_ptr(), center.data_ptr(),
-          (ctypes.c_int * 3)(channels, h, w), _MODE[interpolation])  # fmt: skip
+    _lib.call("b200_rotate_f16_h2", img_chw2.device, out.data_ptr(), img_chw2.data_ptr(), angle.data_ptr(),
+              center.data_ptr(), (ctypes.c_int * 3)(channels, h, w), _MODE[interpolation])  # fmt: skip
     return out
 
 
@@ -135,7 +129,7 @@ def rotate_int8(img_chw4, scale_i, channels, angle, center, scale_o, interpolati
     adt = angle.dtype if torch.is_tensor(angle) and angle.dtype == torch.float16 else torch.float32
     angle, center = _scalars(img_chw4, angle, center, adt)
     out = torch.empty_like(img_chw4)
-    _call("b200_rotate_i8", img_chw4, out.data_ptr(), float(scale_o), img_chw4.data_ptr(), float(scale_i),
-          angle.data_ptr(), center.data_ptr(), int(adt == torch.float16), (ctypes.c_int * 3)(channels, h, w),
-          _MODE[interpolation])  # fmt: skip
+    _lib.call("b200_rotate_i8", img_chw4.device, out.data_ptr(), float(scale_o), img_chw4.data_ptr(), float(scale_i),
+              angle.data_ptr(), center.data_ptr(), int(adt == torch.float16), (ctypes.c_int * 3)(channels, h, w),
+              _MODE[interpolation])  # fmt: skip
     return out

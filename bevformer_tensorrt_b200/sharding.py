@@ -470,9 +470,7 @@ class GroupedSCASampler:
                          (ctypes.c_void_p * n)(*p["flags"]), n, s.my_index, (s.own0 - s.q0) * self.width,
                          (s.own1 - s.own0) * self.width, self.out.data_ptr(), int(self.out_dtype == torch.float16),
                          self.rows * self.width)  # fmt: skip
-        with torch.cuda.device(self.out.device):
-            st = _lib.load().b200_sca_peer_reduce_auto(*p["args"], _lib.current_stream_ptr())
-        _lib.check("b200_sca_peer_reduce_auto", st)
+        _lib.call("b200_sca_peer_reduce_auto", self.out.device, *p["args"])
         return self.out
 
     def _step_overlapped(self):
