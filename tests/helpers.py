@@ -60,6 +60,24 @@ def load_golden_msda(path):
     return cfg, inputs, z["out"]
 
 
+def kernels_recorded(fn, found, tries=3):
+    """Runs ``fn()`` under a CUDA activity trace until ``found(names)`` holds, at most ``tries`` times. Returns (the last
+    result, the kernel names recorded over every try). The trace now and then loses a kernel record: on an H100, about
+    one MSDA backward call in 300 came back without its gather kernel, once without any of its kernels. Since the
+    names of every try are kept, a kernel that should never run is checked against every call made."""
+    from torch.profiler import ProfilerActivity, profile
+
+    names = []
+    for _ in range(tries):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            result = fn()
+            torch.cuda.synchronize()
+        names += [e.name for e in prof.events()]
+        if found(names):
+            break
+    return result, names
+
+
 def make_grid_sampler_inputs(N, C, Hi, Wi, Ho, Wo, seed=0, depth=None, span=15.0):
     """input ~ N(0,1); grid = a regular sweep over [-span, span] (1.5x beyond the image, as the reference test's
     linspace(-15, 15), test_grid_sampler.py:29-36) plus N(0, 0.5) jitter, channel-first [N, 2|3, ...]."""

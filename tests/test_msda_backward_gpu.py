@@ -21,6 +21,7 @@ from bevformer_tensorrt_b200 import _lib
 from bevformer_tensorrt_b200.workloads import CONFIGS, MSDAConfig, make_msda_inputs
 from oracle import msda as omsda
 from oracle.msda_backward import msda_backward_f64
+from tests.helpers import kernels_recorded
 
 NAMES = ("value", "reference_points", "sampling_offsets", "attention_weights")
 
@@ -270,16 +271,13 @@ def test_base_shapes_match_the_oracle(name, dist, dtype):
 @pytest.mark.parametrize("name", ENVELOPE)
 @pytest.mark.parametrize("dist", ["edge", "U"])
 def test_both_kernels_across_the_selection_rule(name, dist, dtype):
-    from torch.profiler import ProfilerActivity, profile
-
     cfg, kernel = ENVELOPE[name]
     inputs = make_msda_inputs(cfg, dist, 31, dtype)
     go = _grad_out(cfg, dtype)
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        _, got = _ours(inputs, go)
-        torch.cuda.synchronize()
-    ran = {e.name for e in prof.events() if "msda_bw_" in e.name}
-    assert any(f"msda_bw_{kernel}_kernel" in n for n in ran), ran
+    took = lambda names: any(f"msda_bw_{kernel}_kernel" in n for n in names)  # noqa: E731
+    (_, got), names = kernels_recorded(lambda: _ours(inputs, go), took)
+    ran = {n for n in names if "msda_bw_" in n}
+    assert took(ran), ran
     assert not any(f"msda_bw_{'generic' if kernel == 'c32' else 'c32'}_kernel" in n for n in ran), ran
     _check_all(got, _oracle(inputs, go), dtype, (name, dist))
 
