@@ -21,6 +21,9 @@ if not _building:
 from .functions import (  # noqa: E402
     TRT_FUNCTIONS,
     bev_point_sampling,
+    bev_pool_v2,
+    bev_pool_v2_2,
+    bev_pool_v2_int8,
     get_reference_points_3d,
     grid_sampler,
     grid_sampler2,
@@ -60,6 +63,9 @@ __all__ = [
     "empty_pinned",
     "TRT_FUNCTIONS",
     "bev_point_sampling",
+    "bev_pool_v2",
+    "bev_pool_v2_2",
+    "bev_pool_v2_int8",
     "get_reference_points_3d",
     "grid_sampler",
     "grid_sampler2",

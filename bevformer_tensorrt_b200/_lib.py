@@ -34,6 +34,7 @@ class TensorDesc(ctypes.Structure):
 
 
 _MSDA_DIMS = [_i] * 8  # batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group
+_BEV_POOL_DIMS = [_i, _i, _i, ctypes.c_longlong, ctypes.c_longlong, _i, _i]  # C, P, I, depth_size, feat_rows, out h, w
 
 SIGNATURES = {
     # name: (restype, argtypes)
@@ -111,6 +112,17 @@ SIGNATURES = {
     "b200_rotate_debug_indices": (_i, [_vp, _vp, _ip, _vp, _vp]),
     "b200_bev_point_sampling": (_i, [_vp, ctypes.POINTER(ctypes.c_double), _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "b200_bev_point_sampling_pillar_heights": (_i, [ctypes.POINTER(ctypes.c_double), _i, ctypes.POINTER(_f)]),
+    # depth, feat, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths, channels, num_points,
+    # num_intervals, depth_size, feat_rows, out_height, out_width, out, stream
+    "b200_bev_pool_f32": (_i, [_vp] * 7 + _BEV_POOL_DIMS + [_vp, _vp]),
+    "b200_bev_pool_f16": (_i, [_vp] * 7 + _BEV_POOL_DIMS + [_vp, _vp]),
+    "b200_bev_pool_i8": (_i, [_vp, _f, _vp, _f] + [_vp] * 5 + _BEV_POOL_DIMS + [_vp, _f, _vp]),
+    "b200_bev_pool_backward_workspace_size": (ctypes.c_size_t, [_i]),
+    "b200_bev_pool_backward_f32": (_i, [_vp] * 9 + _BEV_POOL_DIMS + [_vp, _vp, _vp, ctypes.c_size_t, _vp]),
+    "b200_bev_pool_backward_f16": (_i, [_vp] * 9 + _BEV_POOL_DIMS + [_vp, _vp, _vp, ctypes.c_size_t, _vp]),
+    "b200_bev_pool_enqueue": (_i, [ctypes.POINTER(TensorDesc), ctypes.POINTER(TensorDesc), ctypes.POINTER(_vp),
+                                   ctypes.POINTER(_vp), _vp, _vp, _i, _i]),
+    "b200_bev_pool_supports_format": (_i, [_i, ctypes.POINTER(TensorDesc), _i, _i]),
 }  # fmt: skip
 
 _lib = None

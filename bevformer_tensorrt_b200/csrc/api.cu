@@ -224,4 +224,66 @@ int b200_dcn_enqueue(const b200_tensor_desc *in, const b200_tensor_desc *out, co
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// BEVPoolV2TRT[2]: enqueue / supportsFormatCombination of the reference (bevPoolPlugin.cpp:71-117, :128-143). The
+// reference takes C from feat.d[3], the interval count from interval_starts.d[0] and the output size from the output
+// descriptor, and checks nothing; here every extent the index checks use comes from the descriptors and must agree.
+static long long desc_numel(const b200_dims &d) {
+  if (d.nbDims < 0 || d.nbDims > 8) return -1;
+  long long n = 1;
+  for (int i = 0; i < d.nbDims; ++i) {
+    if (d.d[i] < 0) return -1;
+    n *= d.d[i];
+  }
+  return n;
+}
+
+int b200_bev_pool_enqueue(const b200_tensor_desc *in, const b200_tensor_desc *out, const void *const *inputs,
+                          void *const *outputs, void *workspace, void *stream, int out_height, int out_width) {
+  (void)workspace;
+  if (!in || !out || !inputs || !outputs) return B200_ERR_BAD_PARAM;
+  const b200_dims &fd = in[1].dims;
+  if (fd.nbDims < 1 || fd.nbDims > 8) return B200_ERR_BAD_PARAM;
+  const int C = fd.d[fd.nbDims - 1];
+  const long long depth_size = desc_numel(in[0].dims), feat_size = desc_numel(fd);
+  if (C <= 0 || depth_size < 0 || feat_size < 0) return B200_ERR_BAD_PARAM;
+  for (int i = 2; i < 7; ++i)
+    if (in[i].dims.nbDims != 1) return B200_ERR_BAD_PARAM;
+  const int P = in[2].dims.d[0], I = in[5].dims.d[0];
+  if (in[3].dims.d[0] != P || in[4].dims.d[0] != P || in[6].dims.d[0] != I) return B200_ERR_BAD_PARAM;
+  if (!dims_are(out[0].dims, 1, out_height, out_width, C)) return B200_ERR_BAD_PARAM;
+  const int32_t *idx[5];
+  for (int i = 0; i < 5; ++i) idx[i] = static_cast<const int32_t *>(inputs[2 + i]);
+  const long long rows = feat_size / C;
+  switch (in[0].type) {
+    case 0:
+      return b200_bev_pool_f32(static_cast<const float *>(inputs[0]), static_cast<const float *>(inputs[1]), idx[0],
+                               idx[1], idx[2], idx[3], idx[4], C, P, I, depth_size, rows, out_height, out_width,
+                               static_cast<float *>(outputs[0]), stream);
+    case 1:
+      return b200_bev_pool_f16(inputs[0], inputs[1], idx[0], idx[1], idx[2], idx[3], idx[4], C, P, I, depth_size, rows,
+                               out_height, out_width, outputs[0], stream);
+    case 2:
+      return b200_bev_pool_i8(static_cast<const int8_t *>(inputs[0]), in[0].scale,
+                              static_cast<const int8_t *>(inputs[1]), in[1].scale, idx[0], idx[1], idx[2], idx[3],
+                              idx[4], C, P, I, depth_size, rows, out_height, out_width,
+                              static_cast<int8_t *>(outputs[0]), out[0].scale, stream);
+    default:
+      return B200_ERR_UNSUPPORTED;
+  }
+}
+
+int b200_bev_pool_supports_format(int pos, const b200_tensor_desc *io, int nb_inputs, int nb_outputs) {
+  if (!io || nb_inputs != 7 || nb_outputs != 1 || pos < 0 || pos > 7) return 0;
+  const b200_tensor_desc &d = io[pos];
+  if (d.format != 0) return 0;
+  if (pos == 0) {
+    const b200_dims &fd = io[1].dims;
+    const bool int8_ok = fd.nbDims >= 1 && fd.nbDims <= 8 && fd.d[fd.nbDims - 1] > 0 && fd.d[fd.nbDims - 1] % 4 == 0;
+    return d.type == 0 || d.type == 1 || (d.type == 2 && int8_ok);
+  }
+  if (pos == 1 || pos == 7) return d.type == io[0].type;
+  return d.type == 3;
+}
+
 }  // extern "C"

@@ -9,6 +9,7 @@
 //   GridSampler2DTRT, GridSampler2DTRT2, GridSampler3DTRT, GridSampler3DTRT2   (gridSamplerPlugin.cpp:20-26, :558-561)
 //   ModulatedDeformableConv2dTRT, ModulatedDeformableConv2dTRT2   (modulatedDeformableConv2dPlugin.cpp:19-23, :515-516)
 //   RotateTRT, RotateTRT2                                         (rotatePlugin.cpp:19-21, :216-330)
+//   BEVPoolV2TRT, BEVPoolV2TRT2                                   (bevPoolPlugin.cpp:17-21, :225-383)
 // enqueue() forwards to the C ABI (include/b200_bev_ops.h); nothing is computed here.
 #if __has_include(<NvInfer.h>)
 #include <NvInfer.h>
@@ -24,7 +25,7 @@ using namespace nvinfer1;
 
 static_assert(sizeof(b200_tensor_desc) == sizeof(PluginTensorDesc), "b200_tensor_desc must mirror PluginTensorDesc");
 
-enum class Op { kMSDA, kGridSampler2D, kGridSampler3D, kDCN, kRotate };
+enum class Op { kMSDA, kGridSampler2D, kGridSampler3D, kDCN, kRotate, kBEVPool };
 
 struct Attrs {  // serialised verbatim (the reference serialises the same fields: gridSamplerPlugin.cpp:157-166,
                 // modulatedDeformableConv2dPlugin.cpp:200-211; MSDA serialises nothing, …Plugin.cpp:142-146)
@@ -32,20 +33,40 @@ struct Attrs {  // serialised verbatim (the reference serialises the same fields
   int32_t stride[2] = {1, 1}, pad[2] = {0, 0}, dil[2] = {1, 1}, groups = 1, deform_groups = 1;  // DCN
 };
 
+// BEVPool's attributes live outside Attrs, so the serialisation of every other plugin keeps its size; BEVPool serialises
+// them as the reference does (bevPoolPlugin.cpp:112-119): int32 out_width, then int32 out_height.
+struct BevAttrs {
+  int32_t out_height = 128, out_width = 128;
+};
+
+// A constant dimension expression. The declaration-only mock of the TensorRT API has no IExprBuilder definition; there
+// the overload below, which yields no expression, is chosen, and the shell still compiles.
+template <class B>
+auto dim_constant(B &b, int32_t v, int) -> decltype(b.constant(v)) {
+  return b.constant(v);
+}
+template <class B>
+const IDimensionExpr *dim_constant(B &, int32_t, long) {
+  return nullptr;
+}
+
 class Plugin final : public IPluginV2DynamicExt {
  public:
-  Plugin(Op op, bool v2, const Attrs &a) : op_(op), v2_(v2), a_(a) {}
+  Plugin(Op op, bool v2, const Attrs &a, const BevAttrs &bev = BevAttrs{}) : op_(op), v2_(v2), a_(a), bev_(bev) {}
 
   // ---- IPluginV2DynamicExt
   IPluginV2DynamicExt *clone() const noexcept override {
-    auto *p = new (std::nothrow) Plugin(op_, v2_, a_);
+    auto *p = new (std::nothrow) Plugin(op_, v2_, a_, bev_);
     if (p) p->setPluginNamespace(ns_.c_str());
     return p;
   }
-  DimsExprs getOutputDimensions(int32_t, const DimsExprs *in, int32_t nb, IExprBuilder &) noexcept override {
+  DimsExprs getOutputDimensions(int32_t, const DimsExprs *in, int32_t nb, IExprBuilder &b) noexcept override {
     DimsExprs o{};
     o.nbDims = 4;
-    if (op_ == Op::kRotate) {  // output = img dims [C, H, W] (rotatePlugin.cpp:52-62)
+    if (op_ == Op::kBEVPool) {  // [1, out_height, out_width, feat.d3] (bevPoolPlugin.cpp:41-52)
+      o.d[0] = dim_constant(b, 1, 0), o.d[1] = dim_constant(b, bev_.out_height, 0);
+      o.d[2] = dim_constant(b, bev_.out_width, 0), o.d[3] = in[1].d[3];
+    } else if (op_ == Op::kRotate) {  // output = img dims [C, H, W] (rotatePlugin.cpp:52-62)
       o.nbDims = 3;
       o.d[0] = in[0].d[0], o.d[1] = in[0].d[1], o.d[2] = in[0].d[2];
     } else if (op_ == Op::kMSDA) {  // [value.d0, offsets.d1, value.d2, value.d3] (…Plugin.cpp:48-58)
@@ -64,6 +85,8 @@ class Plugin final : public IPluginV2DynamicExt {
   bool supportsFormatCombination(int32_t pos, const PluginTensorDesc *io, int32_t nbIn, int32_t nbOut) noexcept override {
     if (op_ == Op::kMSDA)
       return b200_msda_supports_format(pos, reinterpret_cast<const b200_tensor_desc *>(io), nbIn, nbOut) != 0;
+    if (op_ == Op::kBEVPool)
+      return b200_bev_pool_supports_format(pos, reinterpret_cast<const b200_tensor_desc *>(io), nbIn, nbOut) != 0;
     if (op_ == Op::kRotate) {  // rotatePlugin.cpp:122-153: img fp32/fp16 linear (kCHW2 for …TRT2) or int8 kCHW4
       const PluginTensorDesc &d = io[pos], &img = io[0];
       if (pos == 0) {
@@ -114,6 +137,10 @@ class Plugin final : public IPluginV2DynamicExt {
     if (op_ == Op::kMSDA)
       return b200_msda_enqueue(reinterpret_cast<const b200_tensor_desc *>(in),
                                reinterpret_cast<const b200_tensor_desc *>(out), inputs, outputs, workspace, stream, v2_);
+    if (op_ == Op::kBEVPool)  // both names run the same kernels
+      return b200_bev_pool_enqueue(reinterpret_cast<const b200_tensor_desc *>(in),
+                                   reinterpret_cast<const b200_tensor_desc *>(out), inputs, outputs, workspace, stream,
+                                   bev_.out_height, bev_.out_width);
     if (op_ == Op::kRotate) {  // inputs: img, angle, center (rotatePlugin.cpp:75-113)
       const int *dims = in[0].dims.d;
       if (in[0].type == DataType::kFLOAT)
@@ -145,6 +172,7 @@ class Plugin final : public IPluginV2DynamicExt {
       case Op::kGridSampler2D: return v2_ ? "GridSampler2DTRT2" : "GridSampler2DTRT";
       case Op::kGridSampler3D: return v2_ ? "GridSampler3DTRT2" : "GridSampler3DTRT";
       case Op::kRotate: return v2_ ? "RotateTRT2" : "RotateTRT";
+      case Op::kBEVPool: return v2_ ? "BEVPoolV2TRT2" : "BEVPoolV2TRT";
       default: return v2_ ? "ModulatedDeformableConv2dTRT2" : "ModulatedDeformableConv2dTRT";
     }
   }
@@ -152,9 +180,17 @@ class Plugin final : public IPluginV2DynamicExt {
   int32_t getNbOutputs() const noexcept override { return 1; }
   int32_t initialize() noexcept override { return 0; }
   void terminate() noexcept override {}
-  size_t getSerializationSize() const noexcept override { return op_ == Op::kMSDA ? 0 : sizeof(Attrs) + sizeof(int32_t); }
+  size_t getSerializationSize() const noexcept override {
+    if (op_ == Op::kBEVPool) return 2 * sizeof(int32_t);
+    return op_ == Op::kMSDA ? 0 : sizeof(Attrs) + sizeof(int32_t);
+  }
   void serialize(void *buf) const noexcept override {
     if (op_ == Op::kMSDA) return;
+    if (op_ == Op::kBEVPool) {
+      std::memcpy(buf, &bev_.out_width, sizeof(int32_t));
+      std::memcpy(static_cast<char *>(buf) + sizeof(int32_t), &bev_.out_height, sizeof(int32_t));
+      return;
+    }
     std::memcpy(buf, &a_, sizeof(Attrs));
     std::memcpy(static_cast<char *>(buf) + sizeof(Attrs), &nb_inputs_, sizeof(int32_t));
   }
@@ -167,6 +203,7 @@ class Plugin final : public IPluginV2DynamicExt {
   Op op_;
   bool v2_;
   Attrs a_;
+  BevAttrs bev_;
   int32_t nb_inputs_ = 5;
   std::string ns_;
 };
@@ -180,6 +217,8 @@ class Creator final : public IPluginCreator {
                  {"align_corners", nullptr, PluginFieldType::kINT32, 1}};
     } else if (op == Op::kRotate) {
       fields_ = {{"interpolation", nullptr, PluginFieldType::kINT32, 1}};
+    } else if (op == Op::kBEVPool) {
+      fields_ = {{"out_height", nullptr, PluginFieldType::kINT32, 1}, {"out_width", nullptr, PluginFieldType::kINT32, 1}};
     } else if (op == Op::kDCN) {
       fields_ = {{"stride", nullptr, PluginFieldType::kINT32, 2},   {"padding", nullptr, PluginFieldType::kINT32, 2},
                  {"dilation", nullptr, PluginFieldType::kINT32, 2}, {"groups", nullptr, PluginFieldType::kINT32, 1},
@@ -193,6 +232,7 @@ class Creator final : public IPluginCreator {
   const PluginFieldCollection *getFieldNames() noexcept override { return &fc_; }
   IPluginV2 *createPlugin(const char *, const PluginFieldCollection *fc) noexcept override {
     Attrs a;
+    BevAttrs bev;
     for (int32_t i = 0; fc && i < fc->nbFields; ++i) {
       const PluginField &f = fc->fields[i];
       const auto *v = static_cast<const int32_t *>(f.data);
@@ -206,12 +246,22 @@ class Creator final : public IPluginCreator {
       else if (n == "dilation") a.dil[0] = v[0], a.dil[1] = f.length > 1 ? v[1] : v[0];
       else if (n == "groups") a.groups = v[0];
       else if (n == "deform_groups") a.deform_groups = v[0];
+      else if (n == "out_height") bev.out_height = v[0];
+      else if (n == "out_width") bev.out_width = v[0];
     }
-    return new (std::nothrow) Plugin(op_, v2_, a);
+    return new (std::nothrow) Plugin(op_, v2_, a, bev);
   }
   IPluginV2 *deserializePlugin(const char *, const void *data, size_t len) noexcept override {
     Attrs a;
     int32_t nb = 5;
+    if (op_ == Op::kBEVPool) {
+      BevAttrs bev;
+      if (len >= 2 * sizeof(int32_t)) {
+        std::memcpy(&bev.out_width, data, sizeof(int32_t));
+        std::memcpy(&bev.out_height, static_cast<const char *>(data) + sizeof(int32_t), sizeof(int32_t));
+      }
+      return new (std::nothrow) Plugin(op_, v2_, a, bev);
+    }
     if (op_ != Op::kMSDA && len >= sizeof(Attrs) + sizeof(int32_t)) {
       std::memcpy(&a, data, sizeof(Attrs));
       std::memcpy(&nb, static_cast<const char *>(data) + sizeof(Attrs), sizeof(int32_t));
@@ -257,6 +307,8 @@ B200_REGISTER(DcnCreator, Op::kDCN, false);
 B200_REGISTER(DcnCreator2, Op::kDCN, true);
 B200_REGISTER(RotateCreator, Op::kRotate, false);
 B200_REGISTER(RotateCreator2, Op::kRotate, true);
+B200_REGISTER(BEVPoolCreator, Op::kBEVPool, false);
+B200_REGISTER(BEVPoolCreator2, Op::kBEVPool, true);
 
 }  // namespace b200_trt
 #endif  // __has_include(<NvInfer.h>)

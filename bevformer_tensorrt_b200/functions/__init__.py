@@ -1,6 +1,7 @@
 """Operator bindings with the reference's names (det2trt/models/functions/__init__.py:1-35) and its function
 registry (det2trt/models/utils/register.py:9-69,86): ``TRT_FUNCTIONS.get("multi_scale_deformable_attn")`` etc."""
 from ..registry import TRT_FUNCTIONS
+from .bev_pool_v2 import bev_pool_v2, bev_pool_v2_2, bev_pool_v2_int8
 from .grid_sampler import grid_sampler, grid_sampler2, grid_sampler_chw2, grid_sampler_int8
 from .modulated_deformable_conv2d import (
     modulated_deformable_conv2d,
@@ -53,3 +54,7 @@ TRT_FUNCTIONS.register_module(module=rotate_int8)
 TRT_FUNCTIONS.register_module(module=get_reference_points_3d)
 TRT_FUNCTIONS.register_module(module=point_sampling_trt)
 TRT_FUNCTIONS.register_module(module=bev_point_sampling)
+
+TRT_FUNCTIONS.register_module(module=bev_pool_v2)
+TRT_FUNCTIONS.register_module(module=bev_pool_v2_2)
+TRT_FUNCTIONS.register_module(module=bev_pool_v2_int8)

@@ -156,3 +156,98 @@ def quantize_per_tensor(x: torch.Tensor):
     scale = scale if scale > 0 else 1.0
     q = torch.clamp(torch.round(x.float() / scale), -128, 127).to(torch.int8)
     return q, scale
+
+
+@dataclass(frozen=True)
+class BevPoolConfig:
+    """One BEVPoolV2 call site: cameras, image size and feature stride, depth bins, channels and the BEV grid."""
+
+    name: str
+    cams: int
+    image_hw: Tuple[int, int]
+    stride: int
+    depth_bins: Tuple[float, float, float]  # (start, stop, step): the frustum's depths, as grid_config["depth"]
+    channels: int
+    grid_lower: Tuple[float, float, float]
+    grid_interval: Tuple[float, float, float]
+    grid_size: Tuple[int, int, int]  # (x, y, z) cells
+
+    @property
+    def feat_hw(self):
+        return self.image_hw[0] // self.stride, self.image_hw[1] // self.stride
+
+    @property
+    def num_depth(self):
+        start, stop, step = self.depth_bins
+        return int(round((stop - start) / step))
+
+    @property
+    def out_hw(self):  # (out_height, out_width) = (y cells, x cells): ranks_bev = y * size_x + x
+        return self.grid_size[1], self.grid_size[0]
+
+
+BEV_POOL_CONFIGS = {
+    # BEVDet-R50 (configs/bevdet/bevdet-r50-cbgs.py): 256x704 input / 16 -> 16x44 features, depth 1..60 m (59 bins),
+    # numC_Trans = 64, a 128x128 grid of 0.8 m cells over +-51.2 m with one z bin over [-5, 3)
+    "bevdet_r50": BevPoolConfig("bevdet_r50", 6, (256, 704), 16, (1.0, 60.0, 1.0), 64, (-51.2, -51.2, -5.0),
+                                (0.8, 0.8, 8.0), (128, 128, 1)),  # fmt: skip
+    # the reference's own op test (det2trt/models/utils/test_trt_ops/test_bev_pool_v2.py): depth [6, 160, 32, 88],
+    # feat [6, 32, 88, 128], a 200x200 grid of 1 m cells over +-100 m
+    "ref_test": BevPoolConfig("ref_test", 6, (512, 1408), 16, (1.0, 161.0, 1.0), 128, (-100.0, -100.0, -5.0),
+                              (1.0, 1.0, 8.0), (200, 200, 1)),  # fmt: skip
+    # a small non-square case that golden fixtures store in full
+    "tiny": BevPoolConfig("tiny", 2, (128, 352), 16, (1.0, 17.0, 1.0), 16, (-12.0, -16.0, -5.0), (1.0, 1.0, 8.0),
+                          (32, 24, 1)),  # fmt: skip
+}
+
+
+def bev_pool_ranks(cfg: BevPoolConfig):
+    """The LSS rank preparation (BEVDet's voxel_pooling_prepare_v2) for a synthetic camera ring, in float64 on the CPU:
+    the frustum (u, v, d) of every feature pixel and depth bin is lifted to the ego frame through the inverse of
+    ``camera_ring_lidar2img``, truncated to voxel coordinates, kept inside the grid, sorted by BEV cell, and cut into one
+    interval per cell. Returns int32 (ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths)."""
+    N, (fh, fw), D = cfg.cams, cfg.feat_hw, cfg.num_depth
+    H_in, W_in = cfg.image_hw
+    start, _, step = cfg.depth_bins
+    d = (start + step * torch.arange(D, dtype=torch.float64)).view(D, 1, 1).expand(D, fh, fw)
+    u = torch.linspace(0, W_in - 1, fw, dtype=torch.float64).view(1, 1, fw).expand(D, fh, fw)
+    v = torch.linspace(0, H_in - 1, fh, dtype=torch.float64).view(1, fh, 1).expand(D, fh, fw)
+    img = torch.stack((u * d, v * d, d, torch.ones_like(d)), -1)  # [D, fh, fw, 4]
+    l2i = camera_ring_lidar2img(N, img_hw=cfg.image_hw, focal=1260.0 * W_in / 1600.0).double()
+    ego = torch.einsum("nij,dhwj->ndhwi", torch.linalg.inv(l2i), img)[..., :3]  # [N, D, fh, fw, 3]
+    coor = ((ego - torch.tensor(cfg.grid_lower, dtype=torch.float64)) /
+            torch.tensor(cfg.grid_interval, dtype=torch.float64)).long().reshape(-1, 3)  # fmt: skip
+    P_all = N * D * fh * fw
+    ranks_depth = torch.arange(P_all, dtype=torch.int64)
+    ranks_feat = torch.arange(N * fh * fw, dtype=torch.int64).view(N, 1, fh, fw).expand(N, D, fh, fw).reshape(-1)
+    sx, sy, sz = cfg.grid_size
+    kept = ((coor[:, 0] >= 0) & (coor[:, 0] < sx) & (coor[:, 1] >= 0) & (coor[:, 1] < sy) & (coor[:, 2] >= 0) &
+            (coor[:, 2] < sz))  # fmt: skip
+    coor, ranks_depth, ranks_feat = coor[kept], ranks_depth[kept], ranks_feat[kept]
+    ranks_bev = coor[:, 2] * sx * sy + coor[:, 1] * sx + coor[:, 0]
+    order = torch.sort(ranks_bev, stable=True).indices
+    ranks_bev, ranks_depth, ranks_feat = ranks_bev[order], ranks_depth[order], ranks_feat[order]
+    first = torch.ones(ranks_bev.numel(), dtype=torch.bool)
+    first[1:] = ranks_bev[1:] != ranks_bev[:-1]
+    starts = torch.nonzero(first).flatten()
+    lengths = torch.diff(starts, append=torch.tensor([ranks_bev.numel()]))
+    return tuple(t.to(torch.int32).contiguous() for t in (ranks_depth, ranks_feat, ranks_bev, starts, lengths))
+
+
+def make_bev_pool_inputs(name: str, seed: int = 0, dtype=torch.float32):
+    """Returns CPU tensors (depth [N, D, fh, fw], feat [N, fh, fw, C], ranks) and (out_height, out_width) for the
+    BEVPoolV2 workload ``name``. depth is a softmax over the depth bins of N(0, 2) logits (what the depth net emits),
+    feat ~ N(0, 1); ranks (bev_pool_ranks) do not depend on the seed."""
+    cfg = BEV_POOL_CONFIGS[name]
+    g = torch.Generator().manual_seed(seed)
+    N, (fh, fw), D, C = cfg.cams, cfg.feat_hw, cfg.num_depth, cfg.channels
+    depth = torch.softmax(2.0 * torch.randn(N, D, fh, fw, generator=g), dim=1)
+    feat = torch.randn(N, fh, fw, C, generator=g)
+    return depth.to(dtype), feat.to(dtype), bev_pool_ranks(cfg), cfg.out_hw
+
+
+def bev_pool_stats(ranks):
+    """Points kept, intervals and the longest interval of a rank set."""
+    lengths = ranks[4]
+    return {"points": int(ranks[0].numel()), "intervals": int(lengths.numel()),
+            "max_interval": int(lengths.max()) if lengths.numel() else 0}  # fmt: skip

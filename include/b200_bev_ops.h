@@ -608,6 +608,74 @@ int b200_dcn_enqueue(const b200_tensor_desc *input_desc, const b200_tensor_desc 
                      void *const *outputs, void *workspace, void *stream, int nb_inputs, const int32_t *stride,
                      const int32_t *padding, const int32_t *dilation, int groups, int deform_groups);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * BEVPoolV2 (plugins BEVPoolV2TRT / BEVPoolV2TRT2; TensorRT/plugin/bev_pool_v2/bevPoolKernel.h, backward
+ * third_party/bev_mmdet3d/ops/bev_pool_v2/src/bev_pool_cuda.cu) — BEVDet's lift-splat pooling:
+ *
+ *   depth            [N, D, H, W]      depth_size = N*D*H*W elements
+ *   feat             [N, H, W, C]      channels last; feat_rows = N*H*W rows of `channels`
+ *   ranks_depth, ranks_feat, ranks_bev   int32 [num_points]
+ *   interval_starts, interval_lengths    int32 [num_intervals]
+ *   out              [1, out_height, out_width, C]
+ *
+ *   out[ranks_bev[s_k], c] = sum_{i = s_k}^{s_k + len_k - 1} feat[ranks_feat[i], c] * depth[ranks_depth[i]]
+ * with s_k = interval_starts[k], len_k = interval_lengths[k]; every cell no interval names is +0 (filled on `stream`).
+ * Contract (what voxel_pooling_prepare_v2 produces): points sorted by ranks_bev, one interval per distinct cell, each
+ * depth element referenced by at most one point. Index safety: [s_k, s_k + len_k) is clipped to [0, num_points); an
+ * interval whose cell ranks_bev[max(s_k, 0)] is outside [0, out_height*out_width) is dropped, and so is a point whose
+ * ranks_depth or ranks_feat is outside its tensor; no input forms an address outside a tensor.
+ * Numerics: FP32 = the reference kernel's FFMA chain in point order, bit for bit. FP16 accumulates in FP32 and rounds
+ * once. INT8 (channels % 4 == 0, else B200_ERR_UNSUPPORTED): exact int32 sum, one multiply by
+ * scale_depth * scale_feat / scale_out (evaluated in float on the host), saturate, round half away from zero.
+ * Pointers of zero-length arrays may be NULL; any other NULL pointer or a negative size is B200_ERR_BAD_PARAM. */
+int b200_bev_pool_f32(const float *depth, const float *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
+                      const int32_t *ranks_bev, const int32_t *interval_starts, const int32_t *interval_lengths,
+                      int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
+                      int out_height, int out_width, float *out, void *stream);
+int b200_bev_pool_f16(const void *depth, const void *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
+                      const int32_t *ranks_bev, const int32_t *interval_starts, const int32_t *interval_lengths,
+                      int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
+                      int out_height, int out_width, void *out, void *stream);
+int b200_bev_pool_i8(const int8_t *depth, float scale_depth, const int8_t *feat, float scale_feat,
+                     const int32_t *ranks_depth, const int32_t *ranks_feat, const int32_t *ranks_bev,
+                     const int32_t *interval_starts, const int32_t *interval_lengths, int channels, int num_points,
+                     int num_intervals, int64_t depth_size, int64_t feat_rows, int out_height, int out_width,
+                     int8_t *out, float scale_out, void *stream);
+
+/* Backward of b200_bev_pool_f32 / _f16, in the input's dtype with FP32 accumulation and no atomics (the same bits on
+ * every run and for every subset of gradients asked for):
+ *   depth_grad[ranks_depth[i]] = sum_c out_grad[cell(i), c] * feat[ranks_feat[i], c]
+ *   feat_grad[f, c]            = sum_{i : ranks_feat[i] = f} out_grad[cell(i), c] * depth[ranks_depth[i]]
+ * where cell(i) is the cell of the interval that pooled point i (= ranks_bev[i] within the contract); both are zero
+ * where no pooled point refers. Either gradient pointer may be NULL (not both). feat_order = the point indices sorted
+ * by ranks_feat with equal keys in index order (a stable argsort, the reference backward's regrouping); needed with
+ * feat_grad only. workspace: b200_bev_pool_backward_workspace_size(num_points) bytes of device memory. */
+size_t b200_bev_pool_backward_workspace_size(int num_points);
+int b200_bev_pool_backward_f32(const float *out_grad, const float *depth, const float *feat, const int32_t *ranks_depth,
+                               const int32_t *ranks_feat, const int32_t *ranks_bev, const int32_t *interval_starts,
+                               const int32_t *interval_lengths, const int32_t *feat_order, int channels, int num_points,
+                               int num_intervals, int64_t depth_size, int64_t feat_rows, int out_height, int out_width,
+                               float *depth_grad, float *feat_grad, void *workspace, size_t workspace_size,
+                               void *stream);
+int b200_bev_pool_backward_f16(const void *out_grad, const void *depth, const void *feat, const int32_t *ranks_depth,
+                               const int32_t *ranks_feat, const int32_t *ranks_bev, const int32_t *interval_starts,
+                               const int32_t *interval_lengths, const int32_t *feat_order, int channels, int num_points,
+                               int num_intervals, int64_t depth_size, int64_t feat_rows, int out_height, int out_width,
+                               void *depth_grad, void *feat_grad, void *workspace, size_t workspace_size,
+                               void *stream);
+
+/* BEVPoolV2TRT[2] (bevPoolPlugin.cpp:71-117): inputs = depth, feat, ranks_depth, ranks_feat, ranks_bev,
+ * interval_starts, interval_lengths; output [1, out_height, out_width, C]. Extents come from the descriptors, which
+ * must agree (index arrays 1-D of matching lengths, output dims = {1, out_height, out_width, feat's last dim}), else
+ * B200_ERR_BAD_PARAM. Dispatch on the depth descriptor's type: fp32, fp16 or int8 (scales from the descriptors). Both
+ * plugin names run the same kernels. Needs no workspace. */
+int b200_bev_pool_enqueue(const b200_tensor_desc *input_desc, const b200_tensor_desc *output_desc,
+                          const void *const *inputs, void *const *outputs, void *workspace, void *stream,
+                          int out_height, int out_width);
+/* supportsFormatCombination mirror: in_out = {the seven inputs, output}; positions 0, 1 and 7 fp32, fp16 or int8
+ * (int8 when C % 4 == 0) kLINEAR of one type, positions 2-6 int32 kLINEAR. */
+int b200_bev_pool_supports_format(int pos, const b200_tensor_desc *in_out, int nb_inputs, int nb_outputs);
+
 #ifdef __cplusplus
 } /* extern "C" */
 #endif
