@@ -33,6 +33,10 @@ class TensorDesc(ctypes.Structure):
     _fields_ = [("dims", Dims), ("type", ctypes.c_int32), ("format", ctypes.c_int32), ("scale", ctypes.c_float)]
 
 
+#: storage dtype of a float entry -> (entry-name suffix, dtype code of the workspace-size queries). The codes are
+#: nvinfer1::DataType's (b200_tensor_desc.type): kFLOAT 0, kHALF 1, kBF16 7.
+DTYPE_CODES = {"float32": ("f32", 0), "float16": ("f16", 1), "bfloat16": ("bf16", 7)}
+
 _MSDA_DIMS = [_i] * 8  # batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group
 _BEV_POOL_DIMS = [_i, _i, _i, ctypes.c_longlong, ctypes.c_longlong, _i, _i]  # C, P, I, depth_size, feat_rows, out h, w
 
@@ -44,11 +48,14 @@ SIGNATURES = {
     "b200_msda_f32": (_i, [_vp] * 5 + _MSDA_DIMS + [_vp, _vp]),
     "b200_msda_f16": (_i, [_vp] * 5 + _MSDA_DIMS + [_vp, _vp]),
     "b200_msda_f16_h2": (_i, [_vp] * 5 + _MSDA_DIMS + [_vp, _vp]),
+    "b200_msda_bf16": (_i, [_vp] * 5 + _MSDA_DIMS + [_vp, _vp]),
     "b200_msda_i8": (_i, [_vp, _f, _vp, _vp, _i, _vp, _f, _vp, _f] + _MSDA_DIMS + [_vp, _f, _vp]),
     "b200_msda_sca_f32": (_i, [_vp] * 6 + _MSDA_DIMS + [_vp, _vp]),
     "b200_msda_sca_f16": (_i, [_vp] * 6 + _MSDA_DIMS + [_vp, _vp]),
+    "b200_msda_sca_bf16": (_i, [_vp] * 6 + _MSDA_DIMS + [_vp, _vp]),
     "b200_msda_sca_shared_f32": (_i, [_vp] * 6 + _MSDA_DIMS + [_vp, _vp]),
     "b200_msda_sca_shared_f16": (_i, [_vp] * 6 + _MSDA_DIMS + [_vp, _vp]),
+    "b200_msda_sca_shared_bf16": (_i, [_vp] * 6 + _MSDA_DIMS + [_vp, _vp]),
     "b200_msda_i8_workspace_size": (ctypes.c_size_t, [_i] * 7),
     "b200_msda_i8_ws": (_i, [_vp, _f, _vp, _vp, _i, _vp, _f, _vp, _f] + _MSDA_DIMS + [_vp, _f, _vp, ctypes.c_size_t, _vp, _vp]),
     "b200_sca_peer_reduce": (_i, [ctypes.POINTER(_vp), ctypes.POINTER(_vp), _i, _i, ctypes.c_uint, ctypes.c_longlong,
@@ -61,15 +68,19 @@ SIGNATURES = {
                                     ctypes.c_longlong, _vp]),
     "b200_msda_f32_trace": (_i, [_vp] * 5 + _MSDA_DIMS + [_vp, _vp, _vp]),
     "b200_msda_f16_trace": (_i, [_vp] * 5 + _MSDA_DIMS + [_vp, _vp, _vp]),
+    "b200_msda_bf16_trace": (_i, [_vp] * 5 + _MSDA_DIMS + [_vp, _vp, _vp]),
     "b200_msda_i8_trace": (_i, [_vp, _f, _vp, _vp, _i, _vp, _f, _vp, _f] + _MSDA_DIMS + [_vp, _f, _vp, _vp]),
     "b200_msda_debug_indices": (_i, [_i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
     "b200_msda_backward_workspace_size": (ctypes.c_size_t, [_i] + _MSDA_DIMS),
     "b200_msda_backward_f32": (_i, [_vp] * 11 + _MSDA_DIMS + [_vp]),
     "b200_msda_backward_f16": (_i, [_vp] * 11 + _MSDA_DIMS + [_vp]),
+    "b200_msda_backward_bf16": (_i, [_vp] * 11 + _MSDA_DIMS + [_vp]),
     "b200_msda_sca_backward_f32": (_i, [_vp] * 12 + _MSDA_DIMS + [_vp]),
     "b200_msda_sca_backward_f16": (_i, [_vp] * 12 + _MSDA_DIMS + [_vp]),
+    "b200_msda_sca_backward_bf16": (_i, [_vp] * 12 + _MSDA_DIMS + [_vp]),
     "b200_msda_sca_shared_backward_f32": (_i, [_vp] * 12 + _MSDA_DIMS + [_vp]),
     "b200_msda_sca_shared_backward_f16": (_i, [_vp] * 12 + _MSDA_DIMS + [_vp]),
+    "b200_msda_sca_shared_backward_bf16": (_i, [_vp] * 12 + _MSDA_DIMS + [_vp]),
     "b200_msda_set_f16_mode": (_i, [_i]),
     "b200_msda_set_f16_path": (_i, [_i]),
     "b200_msda_set_batch_units": (_i, [_i, _i]),
@@ -94,11 +105,13 @@ SIGNATURES = {
     "b200_dcn_i8": (_i, [_vp, _f, _vp, _f, _vp, _i, _vp, _f, _vp, _f, _vp, _f, _vp] + [_i] * 16 + [_vp, _vp]),
     "b200_dcn_f32": (_i, [_vp] * 7 + [_i] * 16 + [_vp, _vp]),
     "b200_dcn_f16": (_i, [_vp] * 7 + [_i] * 16 + [_vp, _vp]),
+    "b200_dcn_bf16": (_i, [_vp] * 7 + [_i] * 16 + [_vp, _vp]),
     "b200_dcn_f16_chw2": (_i, [_vp] * 7 + [_i] * 16 + [_vp, _vp]),
     "b200_dcn_f16_chw2_workspace_size": (ctypes.c_size_t, [_i] * 15),
     "b200_dcn_backward_workspace_size": (ctypes.c_size_t, [_i] * 16),
     "b200_dcn_backward_f32": (_i, [_vp] * 11 + [_i] * 15 + [_vp]),
     "b200_dcn_backward_f16": (_i, [_vp] * 11 + [_i] * 16 + [_vp]),
+    "b200_dcn_backward_bf16": (_i, [_vp] * 11 + [_i] * 15 + [_vp]),
     "b200_grid_sample_set_tile_path": (_i, [_i]),
     "b200_grid_sample_f32": (_i, [_vp, _vp, _vp, _ip, _ip, _ip, _i, _i, _i, _i, _vp]),
     "b200_grid_sample_f16": (_i, [_vp, _vp, _vp, _ip, _ip, _ip, _i, _i, _i, _i, _vp]),
@@ -164,6 +177,15 @@ def call(fn_name: str, device, *args, accept=(B200_OK,)) -> int:
     if status not in accept:
         raise B200OpsError(fn_name, status)
     return status
+
+
+def float_dtype(dtype, fn_name: str):
+    """(entry-name suffix, workspace-query dtype code) of a float storage dtype: ("f32", 0), ("f16", 1) or ("bf16", 7).
+    Any other dtype raises B200OpsError(fn_name, 1), the status of an unsupported dtype."""
+    code = DTYPE_CODES.get(str(dtype).rpartition(".")[2])
+    if code is None:
+        raise B200OpsError(fn_name, 1)
+    return code
 
 
 def launch_count() -> int:

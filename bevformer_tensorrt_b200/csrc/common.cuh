@@ -1,5 +1,6 @@
 // common.cuh — shared device/host helpers for libb200_bev_ops (sm_90a only).
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -58,6 +59,19 @@ __device__ __forceinline__ float2 h2_to_f2(uint32_t u) {
 __device__ __forceinline__ uint32_t f2_to_h2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t *>(&h);
+}
+
+// BF16 is the upper half of an fp32 word, so a packed pair widens exactly with a shift and a mask (no conversion
+// instruction); the store rounds to nearest even once.
+__device__ __forceinline__ float2 bf2_to_f2(uint32_t u) {
+  return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));
+}
+__device__ __forceinline__ uint32_t f2_to_bf2(float a, float b) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t *>(&h);
+}
+__device__ __forceinline__ float bf16_to_f(__nv_bfloat16 v) {
+  return __uint_as_float(static_cast<uint32_t>(__bfloat16_as_ushort(v)) << 16);
 }
 
 // d = a(f16) * b(f16) + c(f32) with one rounding: the product of two fp16 values (11-bit significands) is exact in fp32,

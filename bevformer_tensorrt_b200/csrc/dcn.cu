@@ -13,6 +13,7 @@
 //                      small or odd channel counts, any kernel size).
 // The reference's `cublas_handle` argument is kept in the C ABI for signature compatibility and ignored.
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -75,7 +76,8 @@ static int dcn_forward(const T *input, const T *weight, const T *bias, const T *
   const bool aligned = workspace && reinterpret_cast<uintptr_t>(workspace) % 256 == 0 &&
                        reinterpret_cast<uintptr_t>(input) % 16 == 0 && reinterpret_cast<uintptr_t>(weight) % 16 == 0 &&
                        reinterpret_cast<uintptr_t>(output) % 16 == 0;
-  if (sizeof(T) == 2 && aligned && dcn_fused_enabled() &&
+  // the wgmma kernel reads FP16 bits: BF16 (also 2 bytes) takes the generic kernel
+  if (std::is_same<T, __half>::value && aligned && dcn_fused_enabled() &&
       dcn_fused_supported(channels, channels_out, kk, group, deformable_group))
     return dcn_fused_f16(reinterpret_cast<const __half *>(input), reinterpret_cast<const __half *>(weight),
                          reinterpret_cast<const __half *>(bias), reinterpret_cast<const __half *>(offset),
@@ -216,8 +218,9 @@ size_t b200_dcn_workspace_size(int dtype, int batch, int channels, int height, i
   if (Ho <= 0 || Wo <= 0 || batch <= 0 || channels <= 0) return 0;
   // The generic kernel needs no workspace (the reference sizes a column buffer here, …Conv2dPlugin.cpp:73-115). The
   // fused FP16 path needs the NHWC copy of the input + the permuted weights (channels_out is not an argument of the
-  // reference's formula either; 512 is the largest the fused path takes). Never 0: hosts pass a real pointer.
-  const size_t fused = dtype == 0 ? 0 : dcn_fused_workspace_bytes(batch, channels, height, width, 512, kernel_h * kernel_w);
+  // reference's formula either; 512 is the largest the fused path takes). FP32 (0) and BF16 (7) run the generic kernel
+  // only. Never 0: hosts pass a real pointer.
+  const size_t fused = dtype == 0 || dtype == 7 ? 0 : dcn_fused_workspace_bytes(batch, channels, height, width, 512, kernel_h * kernel_w);
   return fused > 256 ? fused : 256;
 }
 
@@ -324,6 +327,21 @@ int b200_dcn_f16(const void *input, const void *weight, const void *bias, const 
                              channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
                              pad_h, dilation_w, dilation_h, group, deformable_group,
                              static_cast<cudaStream_t>(stream));
+}
+
+// BF16: the generic kernel (fp32 accumulation, one rounding per output); there is no BF16 tensor-core path.
+int b200_dcn_bf16(const void *input, const void *weight, const void *bias, const void *offset, const void *mask,
+                  void *output, void *workspace, int batch, int channels, int height, int width, int channels_out,
+                  int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
+                  int dilation_h, int group, int deformable_group, int im2col_step, void *cublas_handle, void *stream) {
+  (void)im2col_step;
+  (void)cublas_handle;
+  using B = __nv_bfloat16;
+  return dcn_forward<B>(static_cast<const B *>(input), static_cast<const B *>(weight), static_cast<const B *>(bias),
+                        static_cast<const B *>(offset), static_cast<const B *>(mask), static_cast<B *>(output),
+                        workspace, batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h,
+                        pad_w, pad_h, dilation_w, dilation_h, group, deformable_group,
+                        static_cast<cudaStream_t>(stream));
 }
 
 size_t b200_dcn_f16_chw2_workspace_size(int batch, int channels, int height, int width, int channels_out, int kernel_w,

@@ -9,8 +9,8 @@
 //   grad_weight[m, (c,t)] = sum_{b,p} grad_out[m, p] * col[(c,t), p]
 //   grad_bias  [m]        = sum_{b,p} grad_out[m, p]
 // with mmcv's coordinate weights and the forward's index rule (h > -1 && w > -1 && h < H && w < W, floor corners, each
-// corner valid on its own). Everything accumulates in fp32; FP16 storage is converted at load and rounded once at the
-// end. Three hand-written kernels on the FP32 pipe, modelled on dcn_generic.cu (64-pixel tiles, a per-tile sampling
+// corner valid on its own). Everything accumulates in fp32; FP16 / BF16 storage is converted at load and rounded once
+// at the end. Three hand-written kernels on the FP32 pipe, modelled on dcn_generic.cu (64-pixel tiles, a per-tile sampling
 // table, K blocks of KC input channels x the taps), no library GEMM:
 //   * data kernel   — CTA = (image, deformable group, 64-pixel tile, split of the group's channel chunks). Per chunk it
 //                     computes the gc tile from W and grad_out in shared memory, scatters grad_input with atomics, and
@@ -23,6 +23,7 @@
 // So grad_weight, grad_bias, grad_offset and grad_mask are bit-reproducible and do not depend on which other gradients
 // are requested; grad_input is not (float atomics, as in mmcv and torchvision).
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -65,6 +66,10 @@ template <>
 __device__ __forceinline__ float bw_ld<__half>(const __half *p) {
   return __half2float(__ldg(p));
 }
+template <>
+__device__ __forceinline__ float bw_ld<__nv_bfloat16>(const __nv_bfloat16 *p) {
+  return bf16_to_f(__ldg(p));
+}
 template <typename T>
 __device__ __forceinline__ void bw_st(T *p, float v);
 template <>
@@ -74,6 +79,10 @@ __device__ __forceinline__ void bw_st<float>(float *p, float v) {
 template <>
 __device__ __forceinline__ void bw_st<__half>(__half *p, float v) {
   *p = __float2half_rn(v);
+}
+template <>
+__device__ __forceinline__ void bw_st<__nv_bfloat16>(__nv_bfloat16 *p, float v) {
+  *p = __float2bfloat16_rn(v);
 }
 
 // Sampling position of tap t at output pixel pix; `off` / `msk` point at the (image, deformable group) planes.
@@ -402,10 +411,12 @@ __global__ void __launch_bounds__(kThreads) dcn_bw_bias_kernel(const T *gout, T 
   if (threadIdx.x == 0) bw_st(grad_bias + co, sh[0]);
 }
 
-__global__ void dcn_bw_f32_to_f16_kernel(const float *in, __half *out, long long n) {
+// the fp32 grad_input accumulator rounded once to the 2-byte storage type (FP16 or BF16)
+template <typename T>
+__global__ void dcn_bw_f32_round_kernel(const float *in, T *out, long long n) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
-    out[i] = __float2half_rn(in[i]);
+    bw_st(out + i, in[i]);
 }
 
 unsigned grid_for(long long n) { return static_cast<unsigned>(n / 256 + 1 < (1 << 20) ? n / 256 + 1 : (1 << 20)); }
@@ -469,7 +480,7 @@ int dcn_backward(const T *input, const T *weight, const T *offset, const T *mask
                  int height, int width, int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h,
                  int pad_w, int pad_h, int dilation_w, int dilation_h, int group, int deformable_group, int flags,
                  cudaStream_t s) {
-  constexpr bool kF16 = sizeof(T) == 2;
+  constexpr bool kF16 = sizeof(T) == 2;  // FP16 or BF16: grad_input is accumulated in the fp32 workspace
   if (!input || !weight || !offset || !mask || !grad_output || !workspace) return B200_ERR_BAD_PARAM;
   if (flags & ~3) return B200_ERR_BAD_PARAM;
   BwPlan pl{};
@@ -482,7 +493,7 @@ int dcn_backward(const T *input, const T *weight, const T *offset, const T *mask
   if (reinterpret_cast<uintptr_t>(workspace) % 256) return B200_ERR_BAD_PARAM;
   if (flags) {  // the layouts of b200_dcn_f16_ex: its envelope and alignment
     if (reinterpret_cast<uintptr_t>(input) % 16 || reinterpret_cast<uintptr_t>(weight) % 16) return B200_ERR_BAD_PARAM;
-    if (!kF16 || !dcn_fused_supported(channels, channels_out, pl.kk, group, deformable_group)) return B200_ERR_UNSUPPORTED;
+    if (!std::is_same<T, __half>::value || !dcn_fused_supported(channels, channels_out, pl.kk, group, deformable_group)) return B200_ERR_UNSUPPORTED;
   }
   if (!grad_input && !grad_weight && !grad_bias && !grad_offset && !grad_mask) return B200_OK;
 
@@ -509,9 +520,11 @@ int dcn_backward(const T *input, const T *weight, const T *offset, const T *mask
     if (static_cast<long long>(deformable_group) * pl.nsplit > 65535 || batch > 65535) return B200_ERR_UNSUPPORTED;
     dcn_bw_data_kernel<T><<<dim3(ptiles, deformable_group * pl.nsplit, batch), kThreads, pl.smem_data, s>>>(p);
     if ((st = check_launch()) != B200_OK) return st;
-    if (grad_input && kF16) {
-      dcn_bw_f32_to_f16_kernel<<<grid_for(nx), 256, 0, s>>>(p.gin, reinterpret_cast<__half *>(grad_input), nx);
-      if ((st = check_launch()) != B200_OK) return st;
+    if constexpr (kF16) {
+      if (grad_input) {
+        dcn_bw_f32_round_kernel<T><<<grid_for(nx), 256, 0, s>>>(p.gin, grad_input, nx);
+        if ((st = check_launch()) != B200_OK) return st;
+      }
     }
     if (p.om_part) {
       const long long n = static_cast<long long>(batch) * deformable_group * pl.kk * P;
@@ -584,6 +597,22 @@ int b200_dcn_backward_f16(const void *input, const void *weight, const void *off
                               channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
                               pad_h, dilation_w, dilation_h, group, deformable_group, flags,
                               static_cast<cudaStream_t>(stream));
+}
+
+// BF16: every tensor and gradient in bf16, fp32 accumulation; no flags (there is no BF16 fused forward whose layouts
+// it would read).
+int b200_dcn_backward_bf16(const void *input, const void *weight, const void *offset, const void *mask,
+                           const void *grad_output, void *grad_input, void *grad_weight, void *grad_bias,
+                           void *grad_offset, void *grad_mask, void *workspace, int batch, int channels, int height,
+                           int width, int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w,
+                           int pad_h, int dilation_w, int dilation_h, int group, int deformable_group, void *stream) {
+  using B = __nv_bfloat16;
+  return dcn_backward<B>(static_cast<const B *>(input), static_cast<const B *>(weight), static_cast<const B *>(offset),
+                         static_cast<const B *>(mask), static_cast<const B *>(grad_output), static_cast<B *>(grad_input),
+                         static_cast<B *>(grad_weight), static_cast<B *>(grad_bias), static_cast<B *>(grad_offset),
+                         static_cast<B *>(grad_mask), workspace, batch, channels, height, width, channels_out, kernel_w,
+                         kernel_h, stride_w, stride_h, pad_w, pad_h, dilation_w, dilation_h, group, deformable_group, 0,
+                         static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -16,7 +16,7 @@
 //     It is rebuilt only when the K walk enters the next deformable group;
 //   * the B tile (KC*kk x 64 pixels) is sampled straight into shared memory through that table (consecutive threads =
 //     consecutive pixels), the A tile (64 x KC*kk weights) is read k-contiguous and stored transposed;
-//   * fp32 FMAs from shared memory, bias added in the epilogue, FP16 storage converted at load / store only.
+//   * fp32 FMAs from shared memory, bias added in the epilogue, FP16 / BF16 storage converted at load / store only.
 #include "common.cuh"
 
 namespace b200 {
@@ -46,6 +46,10 @@ template <>
 __device__ __forceinline__ float g_ld<__half>(const __half *p) {
   return __half2float(__ldg(p));
 }
+template <>
+__device__ __forceinline__ float g_ld<__nv_bfloat16>(const __nv_bfloat16 *p) {
+  return bf16_to_f(__ldg(p));
+}
 template <typename T>
 __device__ __forceinline__ void g_st(T *p, float v);
 template <>
@@ -55,6 +59,10 @@ __device__ __forceinline__ void g_st<float>(float *p, float v) {
 template <>
 __device__ __forceinline__ void g_st<__half>(__half *p, float v) {
   *p = __float2half_rn(v);
+}
+template <>
+__device__ __forceinline__ void g_st<__nv_bfloat16>(__nv_bfloat16 *p, float v) {
+  *p = __float2bfloat16_rn(v);
 }
 
 template <typename T>
@@ -206,5 +214,9 @@ template int dcn_generic_launch<float>(const float *, const float *, const float
 template int dcn_generic_launch<__half>(const __half *, const __half *, const __half *, const __half *, const __half *,
                                         __half *, int, int, int, int, int, int, int, int, int, int, int, int, int, int, int,
                                         int, int, cudaStream_t);
+template int dcn_generic_launch<__nv_bfloat16>(const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *,
+                                               const __nv_bfloat16 *, const __nv_bfloat16 *, __nv_bfloat16 *, int, int,
+                                               int, int, int, int, int, int, int, int, int, int, int, int, int, int, int,
+                                               cudaStream_t);
 
 }  // namespace b200

@@ -215,6 +215,48 @@ struct Io<__half, MODE> {
   }
 };
 
+// BF16: FP16's lane layout (8 channels = 16 B per lane) and FP16's exact MODE 0 arithmetic: every bf16 word is widened
+// to fp32 exactly (bf2_to_f2: a shift and a mask), fp32 weights, FFMA2, one rounding of the result. No mixed mode.
+template <int MODE>
+struct Io<__nv_bfloat16, MODE> {
+  static_assert(MODE == 0, "BF16 has the exact mode only");
+  static constexpr int kVec = 8, kWt = 4;
+  using Tap = uint4;
+  __device__ static Tap ld(const char *p) { return ldg128(p); }
+  __device__ static void store_zero(__nv_bfloat16 *p) { stg128_stream(p, make_uint4(0u, 0u, 0u, 0u)); }
+  using OffRaw = uint4;
+  __device__ static OffRaw ld_off_raw(const __nv_bfloat16 *p) { return ldg128_stream(p); }
+  __device__ static void decode_off(const OffRaw &a, float, float (&ox)[4], float (&oy)[4]) {
+    const float2 p0 = bf2_to_f2(a.x), p1 = bf2_to_f2(a.y), p2 = bf2_to_f2(a.z), p3 = bf2_to_f2(a.w);
+    ox[0] = p0.x, oy[0] = p0.y, ox[1] = p1.x, oy[1] = p1.y, ox[2] = p2.x, oy[2] = p2.y, ox[3] = p3.x, oy[3] = p3.y;
+  }
+  __device__ static void load_off4(const __nv_bfloat16 *p, float s, float (&ox)[4], float (&oy)[4]) {
+    decode_off(ldg128_stream(p), s, ox, oy);
+  }
+  __device__ static void load_lg4(const __nv_bfloat16 *p, float, float (&lg)[4]) {
+    const uint2 a = ldg64_stream(p);
+    const float2 p0 = bf2_to_f2(a.x), p1 = bf2_to_f2(a.y);
+    lg[0] = p0.x, lg[1] = p0.y, lg[2] = p1.x, lg[3] = p1.y;
+  }
+  __device__ static void pack_w(float (&o)[4], float w00, float w01, float w10, float w11) {
+    o[0] = w00, o[1] = w01, o[2] = w10, o[3] = w11;
+  }
+  __device__ static void fma_point(float (&acc)[8], const Tap (&t)[4], const float (&w)[4]) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t u[4] = {t[k].x, t[k].y, t[k].z, t[k].w};
+      float2 *a2 = reinterpret_cast<float2 *>(acc);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a2[i] = ffma2(bf2_to_f2(u[i]), w[k], a2[i]);
+    }
+  }
+  __device__ static void store(__nv_bfloat16 *p, const float (&acc)[8], float inv_sum, const MsdaParams &) {
+    stg128_stream(p, make_uint4(f2_to_bf2(acc[0] * inv_sum, acc[1] * inv_sum), f2_to_bf2(acc[2] * inv_sum, acc[3] * inv_sum),
+                                f2_to_bf2(acc[4] * inv_sum, acc[5] * inv_sum),
+                                f2_to_bf2(acc[6] * inv_sum, acc[7] * inv_sum)));
+  }
+};
+
 // INT8: 8 channels (8 bytes) per lane, 4 lanes per item like FP16 — same ownership structure, half the tap bytes.
 // Taps are dequantised in registers. int8 -> fp16 is exact (|q| <= 128): flip the sign bit, splice each byte under the
 // exponent byte 0x64 (= 1024 + byte as fp16) with PRMT, subtract 1152 with one packed HADD2 per pair. The product with
@@ -775,6 +817,10 @@ __device__ __forceinline__ float load_as_float<__half>(const __half *p, long lon
   return __half2float(__ldg(p + i));
 }
 template <>
+__device__ __forceinline__ float load_as_float<__nv_bfloat16>(const __nv_bfloat16 *p, long long i, float) {
+  return bf16_to_f(__ldg(p + i));
+}
+template <>
 __device__ __forceinline__ float load_as_float<int8_t>(const int8_t *p, long long i, float s) {
   return static_cast<float>(__ldg(p + i)) * s;
 }
@@ -787,6 +833,10 @@ __device__ __forceinline__ void store_from_float<float>(float *p, long long i, f
 template <>
 __device__ __forceinline__ void store_from_float<__half>(__half *p, long long i, float v, const MsdaParams &) {
   p[i] = __float2half_rn(v);
+}
+template <>
+__device__ __forceinline__ void store_from_float<__nv_bfloat16>(__nv_bfloat16 *p, long long i, float v, const MsdaParams &) {
+  p[i] = __float2bfloat16_rn(v);
 }
 template <>
 __device__ __forceinline__ void store_from_float<int8_t>(int8_t *p, long long i, float v, const MsdaParams &prm) {
@@ -1026,6 +1076,13 @@ static int msda_f16_op(MsdaParams p, int32_t *records, cudaStream_t s) {
   return mixed && !records ? dispatch<__half, __half, 1>(p, s) : dispatch<__half, __half, 0>(p, s);
 }
 
+// BF16 value / offsets / logits / out with FP32 reference points (a bf16 reference point would move the sampling
+// position by up to 2^-9 of the level's extent). FP16's kernel selection; the FP16 mode and path switches do not apply.
+static int msda_bf16_op(MsdaParams p, int32_t *records, cudaStream_t s) {
+  const int st = op_prologue(p, records, s);
+  return st != B200_OK ? st : dispatch<__nv_bfloat16, float, 0>(p, s);
+}
+
 static int msda_i8_op(MsdaParams p, int32_t *records, cudaStream_t s) {
   if (p.C % 4 != 0 || p.P % 4 != 0) return B200_ERR_UNSUPPORTED;  // …Plugin.cpp:151-156
   if (!(p.scale_out > 0.f)) return B200_ERR_BAD_PARAM;
@@ -1085,6 +1142,16 @@ int b200_msda_f16_h2(const void *value, const int32_t *spatial_shapes, const voi
                        num_heads, channels, num_levels, num_query, num_point, points_per_group, out, stream);
 }
 
+int b200_msda_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                   const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size, int num_heads,
+                   int channels, int num_levels, int num_query, int num_point, int points_per_group, void *out,
+                   void *stream) {
+  return msda_bf16_op(make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
+                                  spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
+                                  out),
+                      nullptr, static_cast<cudaStream_t>(stream));
+}
+
 int b200_msda_i8(const int8_t *value, float scale_value, const int32_t *spatial_shapes, const void *reference_points,
                  int ref_is_half, const int8_t *sampling_offsets, float scale_offset, const int8_t *attn_weight,
                  float scale_weight, int batch, int spatial_size, int num_heads, int channels, int num_levels,
@@ -1117,6 +1184,17 @@ int b200_msda_sca_f16(const void *value, const int32_t *spatial_shapes, const vo
   return dispatch<__half, __half, 0, 1>(p, static_cast<cudaStream_t>(stream));
 }
 
+int b200_msda_sca_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                       const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
+                       int spatial_size, int num_heads, int channels, int num_levels, int num_query, int num_point,
+                       int points_per_group, float *accum, void *stream) {
+  MsdaParams p = make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
+                             spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
+                             nullptr);
+  p.mask = bev_mask, p.accum = accum;
+  return dispatch<__nv_bfloat16, float, 0, 1>(p, static_cast<cudaStream_t>(stream));
+}
+
 int b200_msda_sca_shared_f32(const float *value, const int32_t *spatial_shapes, const float *reference_points,
                              const float *sampling_offsets, const float *attn_weight, const float *bev_mask,
                              int batch, int spatial_size, int num_heads, int channels, int num_levels, int num_query,
@@ -1141,6 +1219,18 @@ int b200_msda_sca_shared_f16(const void *value, const int32_t *spatial_shapes, c
   return dispatch<__half, __half, 0, 2>(p, static_cast<cudaStream_t>(stream));
 }
 
+int b200_msda_sca_shared_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                              const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
+                              int spatial_size, int num_heads, int channels, int num_levels, int num_query,
+                              int num_point, int points_per_group, float *slots, void *stream) {
+  MsdaParams p = make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
+                             spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
+                             nullptr);
+  p.mask = bev_mask, p.accum = slots;
+  p.items = static_cast<long long>(num_query) * num_heads;
+  return dispatch<__nv_bfloat16, float, 0, 2>(p, static_cast<cudaStream_t>(stream));
+}
+
 // The plugin ops with the trace switch on: same kernel selection, plus one record per point.
 int b200_msda_f32_trace(const float *value, const int32_t *spatial_shapes, const float *reference_points,
                         const float *sampling_offsets, const float *attn_weight, int batch, int spatial_size,
@@ -1162,6 +1252,17 @@ int b200_msda_f16_trace(const void *value, const int32_t *spatial_shapes, const 
                                  spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
                                  out),
                      records, static_cast<cudaStream_t>(stream));
+}
+
+int b200_msda_bf16_trace(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                         const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size,
+                         int num_heads, int channels, int num_levels, int num_query, int num_point,
+                         int points_per_group, void *out, int32_t *records, void *stream) {
+  if (!records) return B200_ERR_BAD_PARAM;
+  return msda_bf16_op(make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
+                                  spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
+                                  out),
+                      records, static_cast<cudaStream_t>(stream));
 }
 
 int b200_msda_i8_trace(const int8_t *value, float scale_value, const int32_t *spatial_shapes,

@@ -23,7 +23,8 @@
 //     point in range writes zeros and reads nothing else (exact: every d_k is 0).
 //   * msda_bw_generic_kernel — any C / P / G, unaligned tensors: one thread per item, scalar loads and atomics.
 // grad_reference_points: both kernels write one fp32 partial per (item, group) in a fixed order; a second kernel sums
-// the heads in head order. FP16 grad_value: the fp32 accumulator is the workspace, rounded once by a final kernel.
+// the heads in head order. FP16 / BF16 grad_value: the fp32 accumulator is the workspace, rounded once by a final kernel.
+// BF16 reads fp32 reference points and writes an fp32 grad_reference_points (BwRef below); FP32 and FP16 use T.
 //
 // The fused SCA forms (msda.cu, b200_msda_sca_* and b200_msda_sca_shared_*) are differentiated by the same lane-group
 // kernel with an epilogue parameter EPI, as in the forward; grad_slots is fp32 [Q, M*C] for both dtypes:
@@ -77,6 +78,20 @@ struct BwIo<float> {
   }
 };
 template <>
+struct BwIo<__nv_bfloat16> {
+  static constexpr int kVec = 8;
+  __device__ static float ld(const __nv_bfloat16 *p) { return bf16_to_f(__ldg(p)); }
+  __device__ static void st(__nv_bfloat16 *p, float v) { *p = __float2bfloat16_rn(v); }
+  __device__ static void st2(__nv_bfloat16 *p, float a, float b) {
+    *reinterpret_cast<uint32_t *>(p) = f2_to_bf2(a, b);
+  }
+  __device__ static float2 ld2(const __nv_bfloat16 *p) { return bf2_to_f2(ldg32(p)); }
+  __device__ static void unpack(const uint4 &u, float (&v)[8]) {
+    const float2 a = bf2_to_f2(u.x), b = bf2_to_f2(u.y), c = bf2_to_f2(u.z), d = bf2_to_f2(u.w);
+    v[0] = a.x, v[1] = a.y, v[2] = b.x, v[3] = b.y, v[4] = c.x, v[5] = c.y, v[6] = d.x, v[7] = d.y;
+  }
+};
+template <>
 struct BwIo<__half> {
   static constexpr int kVec = 8;
   __device__ static float ld(const __half *p) { return __half2float(__ldg(p)); }
@@ -87,6 +102,17 @@ struct BwIo<__half> {
     const float2 a = h2_to_f2(u.x), b = h2_to_f2(u.y), c = h2_to_f2(u.z), d = h2_to_f2(u.w);
     v[0] = a.x, v[1] = a.y, v[2] = b.x, v[3] = b.y, v[4] = c.x, v[5] = c.y, v[6] = d.x, v[7] = d.y;
   }
+};
+
+// Storage type of the reference points and of their gradient: T, except BF16, which reads and writes them in fp32 (a
+// bf16 reference point would move the sample by up to 2^-9 of the level's extent).
+template <typename T>
+struct BwRef {
+  using type = T;
+};
+template <>
+struct BwRef<__nv_bfloat16> {
+  using type = float;
 };
 
 __device__ __forceinline__ void red_add_v4(float *p, float a, float b, float c, float d) {
@@ -114,6 +140,7 @@ __device__ __forceinline__ void store_ref_partial(float *ref_item, const float (
 template <typename T, int EPI>
 __global__ void __launch_bounds__(kBwThreads, 2) msda_bw_c32_kernel(const MsdaBwParams prm) {
   using IO = BwIo<T>;
+  using R = typename BwRef<T>::type;
   constexpr int C = 32, VEC = IO::kVec, LPI = C / VEC, IPW = 32 / LPI, IPB = IPW * (kBwThreads / 32);
   extern __shared__ float bw_park[];  // [IPB][NP][3]: d, grad_off_x, grad_off_y of every point of the CTA's items
   __shared__ int sH[kBwMaxLevels], sW[kBwMaxLevels], sStart[kBwMaxLevels];
@@ -152,7 +179,7 @@ __global__ void __launch_bounds__(kBwThreads, 2) msda_bw_c32_kernel(const MsdaBw
   for (int bi = 0; bi < num_b; ++bi) {
   const long long bqc = EPI == 2 ? static_cast<long long>(bi) * Q + bq : bq;  // (camera, query) of ref and mask
   const int b = EPI == 2 ? bi : static_cast<int>(bq / Q);
-  const T *ref_bq = static_cast<const T *>(prm.ref) + bqc * 2 * G;
+  const R *ref_bq = static_cast<const R *>(prm.ref) + bqc * 2 * G;
   float *ref_item = EPI == 2 && ref_first ? ref_first + bi * prm.items * G * 2 : ref_first;
   float mk = 1.f;
   bool live = active;  // EPI 1 / 2: and this (camera, query) pair has bev_mask != 0; nothing else of the pair is read
@@ -166,7 +193,7 @@ __global__ void __launch_bounds__(kBwThreads, 2) msda_bw_c32_kernel(const MsdaBw
   float rpx[4], rpy[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const float2 r = EPI == 0 || live ? IO::ld2(ref_bq + 2 * (j % G)) : make_float2(0.f, 0.f);
+    const float2 r = EPI == 0 || live ? BwIo<R>::ld2(ref_bq + 2 * (j % G)) : make_float2(0.f, 0.f);
     rpx[j] = r.x, rpy[j] = r.y;
   }
 
@@ -175,7 +202,7 @@ __global__ void __launch_bounds__(kBwThreads, 2) msda_bw_c32_kernel(const MsdaBw
   if (EPI == 0 || live)
     for (int k = sub; k < NP; k += LPI) {
       const int l = k / P, g = (k - l * P) % G;
-      const float2 r = IO::ld2(ref_bq + 2 * g), o = IO::ld2(off_item + 2 * k);
+      const float2 r = BwIo<R>::ld2(ref_bq + 2 * g), o = IO::ld2(off_item + 2 * k);
       any |= point_record(r.x, r.y, o.x, o.y, sH[l], sW[l]).in_range;
     }
   if (__ballot_sync(kFullMask, any && live) == 0u) {
@@ -360,9 +387,11 @@ __device__ __noinline__ void bw_point_generic(const T *vl, float *acc, const T *
 template <typename T>
 __global__ void __launch_bounds__(kBwThreads) msda_bw_generic_kernel(const MsdaBwParams prm) {
   using IO = BwIo<T>;
+  using R = typename BwRef<T>::type;
   const int M = prm.M, C = prm.C, Q = prm.Q, P = prm.P, G = prm.G, L = prm.L, NP = L * P;
   const T *value = static_cast<const T *>(prm.value), *off = static_cast<const T *>(prm.off);
-  const T *logits = static_cast<const T *>(prm.logits), *ref = static_cast<const T *>(prm.ref);
+  const T *logits = static_cast<const T *>(prm.logits);
+  const R *ref = static_cast<const R *>(prm.ref);
   const long long stp = static_cast<long long>(M) * C;
   for (long long it = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; it < prm.items;
        it += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -385,7 +414,7 @@ __global__ void __launch_bounds__(kBwThreads) msda_bw_generic_kernel(const MsdaB
         const long long lvl = ((static_cast<long long>(b) * prm.S + start) * M + m) * C;
         for (int p = 0; p < P; ++p, ++k) {
           const int g = p % G;
-          const PointRec rec = point_record(IO::ld(ref + bq * 2 * G + 2 * g), IO::ld(ref + bq * 2 * G + 2 * g + 1),
+          const PointRec rec = point_record(BwIo<R>::ld(ref + bq * 2 * G + 2 * g), BwIo<R>::ld(ref + bq * 2 * G + 2 * g + 1),
                                             IO::ld(off + (it * NP + k) * 2), IO::ld(off + (it * NP + k) * 2 + 1), H, W);
           const float a = expf(IO::ld(logits + it * NP + k) - mx) * inv;
           float res[3] = {0.f, 0.f, 0.f};
@@ -425,10 +454,12 @@ __global__ void msda_bw_ref_kernel(const float *part, T *gref, long long nbq, in
   }
 }
 
-__global__ void msda_bw_f32_to_f16_kernel(const float *in, __half *out, long long n) {
+// the fp32 grad_value accumulator rounded once to the 2-byte storage type (FP16 or BF16)
+template <typename T>
+__global__ void msda_bw_f32_round_kernel(const float *in, T *out, long long n) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
-    out[i] = __float2half_rn(in[i]);
+    BwIo<T>::st(out + i, in[i]);
 }
 
 // ---- host ------------------------------------------------------------------------------------------------------------
@@ -470,18 +501,19 @@ bool msda_bw_takes_c32(const MsdaBwParams &p) {
 
 // EPI 0: the plugin op (mask null, gout = grad_out in T). EPI 1 / 2: the fused SCA forms (gout = grad_slots, fp32
 // [Q, M*C]; mask = bev_mask [B, Q]), lane-group kernel only: shapes outside its envelope return B200_ERR_UNSUPPORTED.
-template <typename T, int EPI>
-int msda_backward(const T *value, const int32_t *shapes, const T *ref, const T *off, const T *logits, const float *mask,
-                  const void *gout, T *gvalue, T *gref, T *goff, T *glog, void *workspace, int B, int S, int M, int C,
+template <typename T, int EPI, typename R = typename BwRef<T>::type>
+int msda_backward(const T *value, const int32_t *shapes, const R *ref, const T *off, const T *logits, const float *mask,
+                  const void *gout, T *gvalue, R *gref, T *goff, T *glog, void *workspace, int B, int S, int M, int C,
                   int L, int Q, int P, int G, cudaStream_t s) {
-  constexpr bool kF16 = sizeof(T) == 2;
+  constexpr bool kF16 = sizeof(T) == 2;  // FP16 or BF16: grad_value is accumulated in the fp32 workspace
   if (!value || !shapes || !ref || !off || !logits || !gout || !workspace) return B200_ERR_BAD_PARAM;
   if (EPI != 0 && !mask) return B200_ERR_BAD_PARAM;
   int st = bw_check_dims(B, S, M, C, L, Q, P, G);
   if (st != B200_OK) return st;
-  const void *ptrs[] = {value, ref, off, logits, gvalue, gref, goff, glog};
+  const void *ptrs[] = {value, off, logits, gvalue, goff, glog};
   for (const void *q : ptrs)
     if (reinterpret_cast<uintptr_t>(q) % sizeof(T)) return B200_ERR_BAD_PARAM;
+  if (reinterpret_cast<uintptr_t>(ref) % sizeof(R) || reinterpret_cast<uintptr_t>(gref) % sizeof(R)) return B200_ERR_BAD_PARAM;
   if (reinterpret_cast<uintptr_t>(gout) % (EPI == 0 ? sizeof(T) : sizeof(float)) ||
       reinterpret_cast<uintptr_t>(mask) % 4)
     return B200_ERR_BAD_PARAM;
@@ -515,13 +547,15 @@ int msda_backward(const T *value, const int32_t *shapes, const T *ref, const T *
     msda_bw_generic_kernel<T><<<grid_for(p.items), kBwThreads, 0, s>>>(p);
   }
   if ((st = check_launch()) != B200_OK) return st;
-  if (gvalue && kF16) {
-    msda_bw_f32_to_f16_kernel<<<grid_for(nv), kBwThreads, 0, s>>>(p.gv_acc, reinterpret_cast<__half *>(gvalue), nv);
-    if ((st = check_launch()) != B200_OK) return st;
+  if constexpr (kF16) {
+    if (gvalue) {
+      msda_bw_f32_round_kernel<T><<<grid_for(nv), kBwThreads, 0, s>>>(p.gv_acc, gvalue, nv);
+      if ((st = check_launch()) != B200_OK) return st;
+    }
   }
   if (gref) {
     const long long nbq = static_cast<long long>(B) * Q;
-    msda_bw_ref_kernel<T><<<grid_for(nbq * 2 * G), kBwThreads, 0, s>>>(p.ref_part, gref, nbq, M, 2 * G);
+    msda_bw_ref_kernel<R><<<grid_for(nbq * 2 * G), kBwThreads, 0, s>>>(p.ref_part, gref, nbq, M, 2 * G);
     if ((st = check_launch()) != B200_OK) return st;
   }
   return B200_OK;
@@ -536,10 +570,10 @@ extern "C" {
 
 size_t b200_msda_backward_workspace_size(int dtype, int batch, int spatial_size, int num_heads, int channels,
                                          int num_levels, int num_query, int num_point, int points_per_group) {
-  if ((dtype != 0 && dtype != 1) || bw_check_dims(batch, spatial_size, num_heads, channels, num_levels, num_query,
+  if ((dtype != 0 && dtype != 1 && dtype != 7) || bw_check_dims(batch, spatial_size, num_heads, channels, num_levels, num_query,
                                                   num_point, points_per_group) != B200_OK)
     return 0;
-  return bw_plan(dtype == 1, batch, spatial_size, num_heads, channels, num_query, points_per_group).total;
+  return bw_plan(dtype != 0, batch, spatial_size, num_heads, channels, num_query, points_per_group).total;
 }
 
 int b200_msda_backward_f32(const float *value, const int32_t *spatial_shapes, const float *reference_points,
@@ -621,6 +655,50 @@ int b200_msda_sca_shared_backward_f16(const void *value, const int32_t *spatial_
       static_cast<__half *>(grad_sampling_offsets), static_cast<__half *>(grad_attn_weight), workspace, batch,
       spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
       static_cast<cudaStream_t>(stream));
+}
+
+// BF16: value, offsets, logits, grad_output and their gradients in bf16; reference points and their gradient in fp32.
+int b200_msda_backward_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                            const void *sampling_offsets, const void *attn_weight, const void *grad_output,
+                            void *grad_value, float *grad_reference_points, void *grad_sampling_offsets,
+                            void *grad_attn_weight, void *workspace, int batch, int spatial_size, int num_heads,
+                            int channels, int num_levels, int num_query, int num_point, int points_per_group,
+                            void *stream) {
+  using B = __nv_bfloat16;
+  return msda_backward<B, 0>(
+      static_cast<const B *>(value), spatial_shapes, reference_points, static_cast<const B *>(sampling_offsets),
+      static_cast<const B *>(attn_weight), nullptr, grad_output, static_cast<B *>(grad_value), grad_reference_points,
+      static_cast<B *>(grad_sampling_offsets), static_cast<B *>(grad_attn_weight), workspace, batch, spatial_size,
+      num_heads, channels, num_levels, num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
+}
+
+int b200_msda_sca_backward_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                                const void *sampling_offsets, const void *attn_weight, const float *bev_mask,
+                                const float *grad_slots, void *grad_value, float *grad_reference_points,
+                                void *grad_sampling_offsets, void *grad_attn_weight, void *workspace, int batch,
+                                int spatial_size, int num_heads, int channels, int num_levels, int num_query,
+                                int num_point, int points_per_group, void *stream) {
+  using B = __nv_bfloat16;
+  return msda_backward<B, 1>(
+      static_cast<const B *>(value), spatial_shapes, reference_points, static_cast<const B *>(sampling_offsets),
+      static_cast<const B *>(attn_weight), bev_mask, grad_slots, static_cast<B *>(grad_value), grad_reference_points,
+      static_cast<B *>(grad_sampling_offsets), static_cast<B *>(grad_attn_weight), workspace, batch, spatial_size,
+      num_heads, channels, num_levels, num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
+}
+
+int b200_msda_sca_shared_backward_bf16(const void *value, const int32_t *spatial_shapes,
+                                       const float *reference_points, const void *sampling_offsets,
+                                       const void *attn_weight, const float *bev_mask, const float *grad_slots,
+                                       void *grad_value, float *grad_reference_points, void *grad_sampling_offsets,
+                                       void *grad_attn_weight, void *workspace, int batch, int spatial_size,
+                                       int num_heads, int channels, int num_levels, int num_query, int num_point,
+                                       int points_per_group, void *stream) {
+  using B = __nv_bfloat16;
+  return msda_backward<B, 2>(
+      static_cast<const B *>(value), spatial_shapes, reference_points, static_cast<const B *>(sampling_offsets),
+      static_cast<const B *>(attn_weight), bev_mask, grad_slots, static_cast<B *>(grad_value), grad_reference_points,
+      static_cast<B *>(grad_sampling_offsets), static_cast<B *>(grad_attn_weight), workspace, batch, spatial_size,
+      num_heads, channels, num_levels, num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

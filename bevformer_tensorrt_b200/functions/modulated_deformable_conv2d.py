@@ -28,8 +28,7 @@ def _forward(input, offset, mask, weight, bias, stride, padding, dilation, group
     if input.dim() != 4 or weight.dim() != 4:
         raise ValueError("input must be [N,C,H,W] and weight [Co, C/groups, kh, kw]")
     dt = input.dtype
-    if dt not in (torch.float32, torch.float16):
-        raise _lib.B200OpsError("modulated_deformable_conv2d", 1)
+    suffix, code = _lib.float_dtype(dt, "modulated_deformable_conv2d")
     (sh, sw), (ph, pw), (dh, dw) = _pair(stride), _pair(padding), _pair(dilation)
     n, c, h, w = input.shape
     co, cig, kh, kw = weight.shape
@@ -47,11 +46,10 @@ def _forward(input, offset, mask, weight, bias, stride, padding, dilation, group
         return _forward_fused_f16(lib, input, offset, mask, weight, bias, (sh, sw), (ph, pw), (dh, dw), (ho, wo))
     input, offset, mask, weight = (t.to(dt).contiguous() for t in (input, offset, mask, weight))
     bias_t = bias.to(dt).contiguous() if bias is not None else None
-    ws_bytes = lib.b200_dcn_workspace_size(int(dt == torch.float16), n, c, h, w, kw, kh, sw, sh, pw, ph, dw, dh)
+    ws_bytes = lib.b200_dcn_workspace_size(code, n, c, h, w, kw, kh, sw, sh, pw, ph, dw, dh)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=input.device)
     out = torch.empty(n, co, ho, wo, dtype=dt, device=input.device)
-    name = "b200_dcn_f32" if dt == torch.float32 else "b200_dcn_f16"
-    _lib.call(name, input.device, input.data_ptr(), weight.data_ptr(),
+    _lib.call(f"b200_dcn_{suffix}", input.device, input.data_ptr(), weight.data_ptr(),
               bias_t.data_ptr() if bias_t is not None else None, offset.data_ptr(), mask.data_ptr(), out.data_ptr(),
               workspace.data_ptr(), n, c, h, w, co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups, min(n, 32),
               None)  # fmt: skip
@@ -119,13 +117,14 @@ def _backward(grad_out, input, offset, mask, weight, bias, stride, padding, dila
     the values the forward used (offset, mask, weight and bias cast to the input dtype) and returned in the dtype of
     the tensor the caller passed."""
     dt = input.dtype
+    suffix, code = _lib.float_dtype(dt, "modulated_deformable_conv2d")
     (sh, sw), (ph, pw), (dh, dw) = _pair(stride), _pair(padding), _pair(dilation)
     x, off, msk, wt = (t.to(dt).contiguous() for t in (input, offset, mask, weight))
     go = grad_out.to(dt).contiguous()
     n, c, h, w = x.shape
     co, _, kh, kw = wt.shape
     lib = _lib.load()
-    ws_bytes = lib.b200_dcn_backward_workspace_size(int(dt == torch.float16), n, c, h, w, co, kw, kh, sw, sh, pw, ph, dw,
+    ws_bytes = lib.b200_dcn_backward_workspace_size(code, n, c, h, w, co, kw, kh, sw, sh, pw, ph, dw,
                                                     dh, groups, deform_groups)  # fmt: skip
     if ws_bytes == 0:
         raise _lib.B200OpsError("b200_dcn_backward_workspace_size", 2)
@@ -134,9 +133,8 @@ def _backward(grad_out, input, offset, mask, weight, bias, stride, padding, dila
     like = [x, wt, go.new_empty(co), off, msk]
     grads = [torch.empty_like(t, memory_format=torch.contiguous_format) if k else None for k, t in zip(want, like)]
     ptr = [g.data_ptr() if g is not None else None for g in grads]
-    name = "b200_dcn_backward_f32" if dt == torch.float32 else "b200_dcn_backward_f16"
-    flags = [] if dt == torch.float32 else [0]
-    _lib.call(name, x.device, x.data_ptr(), wt.data_ptr(), off.data_ptr(), msk.data_ptr(), go.data_ptr(), *ptr,
+    flags = [0] if dt == torch.float16 else []  # the layout flags of the FP16 entry: plain NCHW, unpacked weights
+    _lib.call(f"b200_dcn_backward_{suffix}", x.device, x.data_ptr(), wt.data_ptr(), off.data_ptr(), msk.data_ptr(), go.data_ptr(), *ptr,
               workspace.data_ptr(), n, c, h, w, co, kw, kh, sw, sh, pw, ph, dw, dh, groups, deform_groups, *flags)
     gi, gw, gb, go_, gm = grads
     cast = lambda g, t: g.to(t.dtype) if g is not None else None  # noqa: E731
@@ -174,7 +172,9 @@ _ModulatedDeformableConv2dFunction2 = _make("ModulatedDeformableConv2dTRT2")
 
 def modulated_deformable_conv2d(input, offset, mask, weight, bias=None, stride=1, padding=0, dilation=1, groups=1,
                                 deform_groups=1):
-    """Plugin ModulatedDeformableConv2dTRT (FP32 / FP16). Same contract as the reference wrapper (:208-248)."""
+    """Plugin ModulatedDeformableConv2dTRT (FP32 / FP16 / BF16). Same contract as the reference wrapper (:208-248).
+    Offset, mask, weight and bias are cast to the input's dtype; gradients come back in each argument's own dtype. BF16
+    runs the generic kernel (csrc/dcn_generic.cu) for every shape."""
     return _ModulatedDeformableConv2dFunction.apply(input, offset, mask, weight, bias, stride, padding, dilation,
                                                     groups, deform_groups)  # fmt: skip
 

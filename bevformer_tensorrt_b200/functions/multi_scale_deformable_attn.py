@@ -100,8 +100,8 @@ def autotune_msda(value, value_spatial_shapes, reference_points, sampling_offset
     distribution (dense sampling is bound by the L1 line rate and wants warps; camera-ring inputs are latency-bound and
     want loads in flight), which the op cannot know from its arguments. Returns a report dict
     ``{"chosen": name, "ms": {name: median ms}, "rejected": [names]}``."""
-    if not value.is_cuda or value.dtype not in (torch.float16, torch.float32):
-        raise ValueError("autotune_msda: FP16 / FP32 CUDA tensors only (the INT8 op has a single launch shape)")
+    if not value.is_cuda or value.dtype not in (torch.float16, torch.bfloat16, torch.float32):
+        raise ValueError("autotune_msda: FP32 / FP16 / BF16 CUDA tensors only (the INT8 op has a single launch shape)")
     args = (value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights)
     set_msda_launch_shape("default")
     base = multi_scale_deformable_attn(*args)
@@ -181,7 +181,8 @@ def set_msda_launch_shape(name: str):
 
 class _Prepared(NamedTuple):
     """The tensors an MSDA entry reads — contiguous, int32 level shapes, reference points / offsets / logits in value's
-    dtype (INT8: as given) — and the entry's eight dimension arguments (_lib._MSDA_DIMS)."""
+    dtype (BF16: reference points in FP32; INT8: as given) — and the entry's eight dimension arguments
+    (_lib._MSDA_DIMS)."""
 
     value: torch.Tensor
     shapes: torch.Tensor
@@ -196,8 +197,9 @@ class _Prepared(NamedTuple):
 
 def _prepare(name, value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, dtype,
              bev_mask=None):
-    """Checks the inputs of the op ``name`` and makes them what its C entry reads. ``dtype``: value's dtype, FP32 or
-    FP16, which reference points, offsets and logits are cast to; None (INT8) casts nothing. ``bev_mask`` is given by the
+    """Checks the inputs of the op ``name`` and makes them what its C entry reads. ``dtype``: value's dtype, FP32, FP16
+    or BF16, which offsets and logits are cast to, and reference points too except for BF16, whose entries read them in
+    FP32; None (INT8) casts nothing. ``bev_mask`` is given by the
     camera-shared form only: its offsets and logits are ONE copy for all cameras and num_query is read from the mask.
     Otherwise they are ``bs`` copies and num_query is sampling_offsets.shape[1], the reference plugin's rule."""
     if not value.is_cuda:
@@ -223,9 +225,10 @@ def _prepare(name, value, value_spatial_shapes, reference_points, sampling_offse
     if reference_points.numel() != bs * num_query * points_per_group * 2:
         raise ValueError("reference_points does not match [bs, num_query, 1, 2*points_per_group]")
     if dtype is not None:
-        if dtype not in (torch.float32, torch.float16):
-            raise _lib.B200OpsError(name, 1)
-        reference_points = _cast(reference_points, dtype)
+        _lib.float_dtype(dtype, name)
+        # bf16 has 8 significant bits: a normalised reference point near 0.9 would move by up to 2^-9 of the level's
+        # extent (0.4 px on a 200-wide BEV plane). A bf16 input is cast up, which is exact.
+        reference_points = _cast(reference_points, torch.float32 if dtype == torch.bfloat16 else dtype)
         sampling_offsets = _cast(sampling_offsets, dtype)
         attention_weights = _cast(attention_weights, dtype)
     dims = (bs, num_keys, num_heads, channels, num_levels, num_query, all_points // num_levels, points_per_group)
@@ -281,7 +284,8 @@ def _launch_int8(p, scales, out, records=None):
 
 
 def _msda_forward(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, use_h2, out=None):
-    """The FP32 / FP16 plugin op. Returns its output and the prepared inputs the kernel read (for the backward)."""
+    """The FP32 / FP16 / BF16 plugin op. Returns its output and the prepared inputs the kernel read (for the
+    backward)."""
     dt = value.dtype
     p = _prepare("multi_scale_deformable_attn", value, value_spatial_shapes, reference_points, sampling_offsets,
                  attention_weights, dt)  # fmt: skip
@@ -290,10 +294,10 @@ def _msda_forward(value, value_spatial_shapes, reference_points, sampling_offset
         out = torch.empty(bs, num_query, num_heads, channels, dtype=dt, device=value.device)
     elif out.dtype != dt or not out.is_contiguous() or out.numel() != bs * num_query * num_heads * channels:
         raise ValueError("out must be a contiguous [bs, num_query, num_heads, channels] tensor of value's dtype")
-    if dt == torch.float32:
-        name = "b200_msda_f32"
-    else:
+    if dt == torch.float16:
         name = "b200_msda_f16_h2" if use_h2 and channels % 2 == 0 else "b200_msda_f16"
+    else:
+        name = f"b200_msda_{_lib.float_dtype(dt, 'multi_scale_deformable_attn')[0]}"
     _lib.call(name, value.device, *p.ptrs(), *p.dims, out.data_ptr())
     return out, p
 
@@ -307,18 +311,19 @@ def _save(ctx, p, inputs, *extra):
 
 
 def _backward_launch(prefix, p, args, needs, accept=(0,)):
-    """Runs the backward entry ``{prefix}_backward_{f32|f16}`` — b200_msda_, b200_msda_sca_ or b200_msda_sca_shared_ —
+    """Runs the backward entry ``{prefix}_backward_{f32|f16|bf16}`` — b200_msda_, b200_msda_sca_ or b200_msda_sca_shared_ —
     on the forward's inputs ``p``. ``args``: the tensors the entry takes between the logits and the gradients (grad_out;
     bev_mask and grad_slots for the fused forms). ``needs``: the op's ``needs_input_grad``, which selects the value,
     reference-point, offset and logit gradients to compute. Returns them (None where not wanted), or None when the entry
     declined with a non-zero status in ``accept``."""
     dt, dev = p.value.dtype, p.value.device
-    ws_bytes = _lib.load().b200_msda_backward_workspace_size(int(dt == torch.float16), *p.dims)
+    suffix, code = _lib.float_dtype(dt, prefix)
+    ws_bytes = _lib.load().b200_msda_backward_workspace_size(code, *p.dims)
     if ws_bytes == 0:
         raise _lib.B200OpsError("b200_msda_backward_workspace_size", 2)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
     grads = [torch.empty_like(t) if needs[i] else None for i, t in ((0, p.value), (2, p.ref), (3, p.off), (4, p.w))]
-    name = f"{prefix}_backward_{'f32' if dt == torch.float32 else 'f16'}"
+    name = f"{prefix}_backward_{suffix}"
     st = _lib.call(name, dev, *p.ptrs(), *[t.data_ptr() for t in args],
                    *[g.data_ptr() if g is not None else None for g in grads], ws.data_ptr(), *p.dims, accept=accept)
     return None if st else grads
@@ -389,14 +394,17 @@ _multi_scale_deformable_attn_gpu2 = _MultiScaleDeformableAttnFunction2.apply
 
 
 def multi_scale_deformable_attn(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights):
-    """Plugin MultiScaleDeformableAttnTRT (FP32 / FP16). Same contract as the reference wrapper (:150-182)."""
+    """Plugin MultiScaleDeformableAttnTRT (FP32 / FP16 / BF16). Same contract as the reference wrapper (:150-182).
+    BF16 reads the reference points in FP32 (a bf16 tensor is cast up) and returns grad_reference_points in the
+    dtype the caller passed."""
     assert value.is_cuda
     return _multi_scale_deformable_attn_gpu(value, value_spatial_shapes, reference_points, sampling_offsets,
                                             attention_weights)  # fmt: skip
 
 
 def multi_scale_deformable_attn2(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights):
-    """Plugin MultiScaleDeformableAttnTRT2 (FP32 / FP16 as half2). Same contract as the reference wrapper (:185-217)."""
+    """Plugin MultiScaleDeformableAttnTRT2 (FP32 / FP16 as half2 / BF16). Same contract as the reference wrapper
+    (:185-217)."""
     assert value.is_cuda
     return _multi_scale_deformable_attn_gpu2(value, value_spatial_shapes, reference_points, sampling_offsets,
                                              attention_weights)  # fmt: skip
@@ -449,7 +457,7 @@ def _sca_forward(value, value_spatial_shapes, reference_points, sampling_offsets
         raise ValueError("accum must be a contiguous float32 [num_query, heads*channels] tensor")
     else:
         res = accum
-    name = f"b200_msda_{form}_{'f32' if dt == torch.float32 else 'f16'}"
+    name = f"b200_msda_{form}_{_lib.float_dtype(dt, form)[0]}"
     fused = _lib.call(name, value.device, *p.ptrs(), mask.data_ptr(), *p.dims, res.data_ptr(), accept=(0, 1)) == 0
     if not fused:
         # shapes the fused kernel does not take (e.g. channels != 32, more than 64 points, unaligned tensors): the plugin
@@ -579,7 +587,7 @@ def msda_sampling_indices(value_spatial_shapes, reference_points, sampling_offse
 def msda_trace(value, value_spatial_shapes, reference_points, sampling_offsets, attention_weights, scales=None):
     """The production MSDA kernel with its trace switch on. Returns ``(out, records)``: ``out`` as the plugin op computes
     it and int32 records [bs, nq, heads, L*P, 4] = {in_range, h_low, w_low, tap_mask} written by the gather kernel itself
-    while it samples (C entries b200_msda_{f32,f16,i8}_trace). ``scales`` = (scale_value, scale_offset, scale_weight,
+    while it samples (C entries b200_msda_{f32,f16,bf16,i8}_trace). ``scales`` = (scale_value, scale_offset, scale_weight,
     scale_out) selects the INT8 kernel (int8 value / offsets / logits, float or half reference points)."""
     assert value.is_cuda
     dt = value.dtype
@@ -591,6 +599,6 @@ def msda_trace(value, value_spatial_shapes, reference_points, sampling_offsets, 
     if dt == torch.int8:
         _launch_int8(p, scales, out, rec)
     else:
-        name = "b200_msda_f32_trace" if dt == torch.float32 else "b200_msda_f16_trace"
+        name = f"b200_msda_{_lib.float_dtype(dt, 'msda_trace')[0]}_trace"
         _lib.call(name, value.device, *p.ptrs(), *p.dims, out.data_ptr(), rec.data_ptr())
     return out, rec

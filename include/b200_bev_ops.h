@@ -72,6 +72,16 @@ int b200_msda_f16_h2(const void *value, const int32_t *spatial_shapes, const voi
                      int num_heads, int channels, int num_levels, int num_query, int num_point, int points_per_group,
                      void *out, void *stream);
 
+/* BF16 (beyond the reference, which has no BF16 plugin): value, sampling_offsets, attn_weight and out are
+ * __nv_bfloat16; reference_points are FP32 (bf16's 8 significant bits would move a normalised point by up to 2^-9 of
+ * the level's extent). Arithmetic = the FP16 entry's exact mode: every bf16 element widened to FP32 exactly, FP32 index
+ * arithmetic and accumulation, one rounding of the result (round to nearest even). Same kernel selection and launch
+ * shapes as b200_msda_f16; b200_msda_set_f16_mode / _set_f16_path do not apply. */
+int b200_msda_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                   const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size, int num_heads,
+                   int channels, int num_levels, int num_query, int num_point, int points_per_group, void *out,
+                   void *stream);
+
 /* replaces ms_deformable_im2col_cuda_int8<float> / <__half2> — …Kernel.h:29-38, .cu:1172-1218.
  * value / offsets / attn_weight / out are int8 with per-tensor scales (real = q * scale, TensorRT PTQ convention,
  * …Plugin.cpp:75-77); reference_points are float (ref_is_half == 0) or __half (ref_is_half != 0).
@@ -98,6 +108,11 @@ int b200_msda_sca_f16(const void *value, const int32_t *spatial_shapes, const vo
                       const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
                       int spatial_size, int num_heads, int channels, int num_levels, int num_query, int num_point,
                       int points_per_group, float *accum, void *stream);
+/* BF16 value / offsets / logits, FP32 reference points (see b200_msda_bf16). */
+int b200_msda_sca_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                       const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
+                       int spatial_size, int num_heads, int channels, int num_levels, int num_query, int num_point,
+                       int points_per_group, float *accum, void *stream);
 
 /* Camera-shared form of the same fused op. SpatialCrossAttention repeats the BEV query for every camera before the
  * sampling_offsets / attention_weights Linear layers (spatial_cross_attention.py:254 `query.repeat(num_cams, 1, 1)`), so
@@ -116,6 +131,10 @@ int b200_msda_sca_shared_f16(const void *value, const int32_t *spatial_shapes, c
                              const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
                              int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                              int num_point, int points_per_group, float *slots, void *stream);
+int b200_msda_sca_shared_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                              const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
+                              int spatial_size, int num_heads, int channels, int num_levels, int num_query,
+                              int num_point, int points_per_group, float *slots, void *stream);
 
 /* ---- Second-generation INT8 MSDA path (csrc/msda_v2.cu): channels == 32, 16 <= num_levels*num_point <= 32 ----
  * Same operator, same semantics and argument meaning as b200_msda_i8, with one addition to the signature: the caller
@@ -196,6 +215,10 @@ int b200_msda_f16_trace(const void *value, const int32_t *spatial_shapes, const 
                         const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size,
                         int num_heads, int channels, int num_levels, int num_query, int num_point,
                         int points_per_group, void *out, int32_t *records, void *stream);
+int b200_msda_bf16_trace(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                         const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size,
+                         int num_heads, int channels, int num_levels, int num_query, int num_point,
+                         int points_per_group, void *out, int32_t *records, void *stream);
 int b200_msda_i8_trace(const int8_t *value, float scale_value, const int32_t *spatial_shapes,
                        const void *reference_points, int ref_is_half, const int8_t *sampling_offsets,
                        float scale_offset, const int8_t *attn_weight, float scale_weight, int batch, int spatial_size,
@@ -231,7 +254,7 @@ int b200_msda_debug_indices(int dtype, const int32_t *spatial_shapes, const void
  * Kernels: csrc/msda_backward.cu. channels == 32 with num_point % 4 == 0, points_per_group in {1, 2, 4},
  * num_levels * num_point <= 64 and 16-byte aligned tensors runs the lane-group kernel; every other shape the forward
  * accepts runs a one-thread-per-item kernel. There is no INT8 backward. */
-size_t b200_msda_backward_workspace_size(int dtype /* 0 f32, 1 f16 */, int batch, int spatial_size, int num_heads,
+size_t b200_msda_backward_workspace_size(int dtype /* 0 f32, 1 f16, 7 bf16 */, int batch, int spatial_size, int num_heads,
                                          int channels, int num_levels, int num_query, int num_point,
                                          int points_per_group);
 int b200_msda_backward_f32(const float *value, const int32_t *spatial_shapes, const float *reference_points,
@@ -246,6 +269,16 @@ int b200_msda_backward_f16(const void *value, const int32_t *spatial_shapes, con
                            void *grad_attn_weight, void *workspace, int batch, int spatial_size, int num_heads,
                            int channels, int num_levels, int num_query, int num_point, int points_per_group,
                            void *stream);
+/* BF16 (b200_msda_bf16): value, offsets, logits, grad_output and their gradients are __nv_bfloat16, reference_points and
+ * grad_reference_points FP32. As FP16: FP32 accumulation (grad_value in the workspace), one rounding per gradient.
+ * Workspace: b200_msda_backward_workspace_size(7, ...) — the dtype codes follow nvinfer1::DataType (7 = kBF16; 2 is
+ * kINT8, which has no backward and keeps returning 0) — the FP16 size. */
+int b200_msda_backward_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                            const void *sampling_offsets, const void *attn_weight, const void *grad_output,
+                            void *grad_value, float *grad_reference_points, void *grad_sampling_offsets,
+                            void *grad_attn_weight, void *workspace, int batch, int spatial_size, int num_heads,
+                            int channels, int num_levels, int num_query, int num_point, int points_per_group,
+                            void *stream);
 
 /* Backward of the fused SCA forms b200_msda_sca_* (camera-summed) and b200_msda_sca_shared_* (camera-shared), with the
  * conventions of b200_msda_backward_* (NULL gradient = not computed, requested gradients overwritten, argument errors
@@ -286,6 +319,20 @@ int b200_msda_sca_shared_backward_f16(const void *value, const int32_t *spatial_
                                       void *grad_sampling_offsets, void *grad_attn_weight, void *workspace, int batch,
                                       int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                                       int num_point, int points_per_group, void *stream);
+/* BF16 forms: dtypes as in b200_msda_backward_bf16 (FP32 reference points and their gradient). */
+int b200_msda_sca_backward_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
+                                const void *sampling_offsets, const void *attn_weight, const float *bev_mask,
+                                const float *grad_slots, void *grad_value, float *grad_reference_points,
+                                void *grad_sampling_offsets, void *grad_attn_weight, void *workspace, int batch,
+                                int spatial_size, int num_heads, int channels, int num_levels, int num_query,
+                                int num_point, int points_per_group, void *stream);
+int b200_msda_sca_shared_backward_bf16(const void *value, const int32_t *spatial_shapes,
+                                       const float *reference_points, const void *sampling_offsets,
+                                       const void *attn_weight, const float *bev_mask, const float *grad_slots,
+                                       void *grad_value, float *grad_reference_points, void *grad_sampling_offsets,
+                                       void *grad_attn_weight, void *workspace, int batch, int spatial_size,
+                                       int num_heads, int channels, int num_levels, int num_query, int num_point,
+                                       int points_per_group, void *stream);
 
 /* Selects the FP16 accumulate flavour for b200_msda_f16*. 0 (default) = exact: taps widened to FP32, FP32 weights,
  * packed FP32 FMA (FFMA2) — meets the 1e-3 max-abs parity bar everywhere. 1 = mixed: FP16 tap x FP16 weight -> FP32
@@ -478,7 +525,7 @@ int b200_bev_point_sampling_pillar_heights(const double *pc_range, int num_point
  * Argument order = the reference launcher ModulatedDeformConvForwardCUDAKernel<T> (…Conv2dKernel.h:11-19).
  * FP16 accumulates the GEMM in FP32 (the reference accumulates in FP16, common/cuda_helper.cu:101-110).
  * ---------------------------------------------------------------------------------------------------------- */
-size_t b200_dcn_workspace_size(int dtype /* 0 f32, 1 f16 */, int batch, int channels, int height, int width,
+size_t b200_dcn_workspace_size(int dtype /* 0 f32, 1 f16, 7 bf16 */, int batch, int channels, int height, int width,
                                int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h,
                                int dilation_w, int dilation_h);
 
@@ -529,7 +576,7 @@ int b200_dcn_f16_ex(const void *input, const void *weight, const void *bias, con
  * yet; b200_dcn_set_fused does not affect it), no library GEMM. NHWC input and packed weights are read in place, so a
  * caller holding the forward's layouts needs no conversion; on this path the plain layouts are the faster ones (at
  * [6,256,58,100] 3x3 on an H100: data kernel +5 % with packed weights, both kernels +15..40 % with an NHWC input). */
-size_t b200_dcn_backward_workspace_size(int dtype /* 0 f32, 1 f16 */, int batch, int channels, int height, int width,
+size_t b200_dcn_backward_workspace_size(int dtype /* 0 f32, 1 f16, 7 bf16 */, int batch, int channels, int height, int width,
                                         int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h,
                                         int pad_w, int pad_h, int dilation_w, int dilation_h, int group,
                                         int deformable_group);
@@ -544,6 +591,13 @@ int b200_dcn_backward_f16(const void *input, const void *weight, const void *off
                           int width, int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w,
                           int pad_h, int dilation_w, int dilation_h, int group, int deformable_group, int flags,
                           void *stream);
+/* BF16: the FP32 entry's arguments (no flags), every tensor and gradient __nv_bfloat16, FP32 accumulation with grad_input
+ * in the workspace (b200_dcn_backward_workspace_size(7, ...) = the FP16 size), one rounding per gradient. */
+int b200_dcn_backward_bf16(const void *input, const void *weight, const void *offset, const void *mask,
+                           const void *grad_output, void *grad_input, void *grad_weight, void *grad_bias,
+                           void *grad_offset, void *grad_mask, void *workspace, int batch, int channels, int height,
+                           int width, int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w,
+                           int pad_h, int dilation_w, int dilation_h, int group, int deformable_group, void *stream);
 
 /* replaces ModulatedDeformConvForwardCUDAKernel_int8<float> / <__half> — …Conv2dKernel.h:21-29, .cu:897-978.
  * input int8 kCHW4 [batch, channels/4, H, W, 4], weight int8 kCHW4 [channels_out, channels/4, kh, kw, 4], offset / mask
@@ -570,6 +624,15 @@ int b200_dcn_f16(const void *input, const void *weight, const void *bias, const 
                  void *output, void *workspace, int batch, int channels, int height, int width, int channels_out,
                  int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
                  int dilation_h, int group, int deformable_group, int im2col_step, void *cublas_handle, void *stream);
+
+/* BF16 (beyond the reference): every tensor __nv_bfloat16, on the generic kernel (csrc/dcn_generic.cu) for every shape
+ * — there is no BF16 tensor-core path. Each element widened to FP32 exactly, FP32 accumulation, one rounding per output.
+ * workspace: b200_dcn_workspace_size(7, ...) bytes (dtype codes follow nvinfer1::DataType:
+ * 7 = kBF16). */
+int b200_dcn_bf16(const void *input, const void *weight, const void *bias, const void *offset, const void *mask,
+                  void *output, void *workspace, int batch, int channels, int height, int width, int channels_out,
+                  int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
+                  int dilation_h, int group, int deformable_group, int im2col_step, void *cublas_handle, void *stream);
 
 /* FP16 in TensorRT's kCHW2 packets — what the …TRT2 plugin negotiates (…Conv2dPlugin.cpp:222-250: input, offset and
  * weight as __half2 packets [N, ceil(C/2), H, W, 2]; mask, bias and output linear). Replaces
