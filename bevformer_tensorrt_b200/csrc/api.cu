@@ -1,6 +1,7 @@
 // api.cu — library-level C ABI: identification, status strings, launch counter, and the plugin-shaped
 // enqueue / supportsFormatCombination mirrors for MSDA (reference: multiScaleDeformableAttnPlugin.cpp:71-189).
 #include "common.cuh"
+#include "dcn_geometry.cuh"
 
 namespace b200 {
 std::atomic<unsigned long long> g_launch_count{0};
@@ -10,7 +11,7 @@ using namespace b200;
 
 extern "C" {
 
-const char *b200_bev_ops_version(void) { return "b200_bev_ops 0.1.0 sm_90a"; }
+const char *b200_bev_ops_version(void) { return "b200_bev_ops 0.1.1 sm_90a"; }
 
 const char *b200_status_string(int status) {
   switch (status) {
@@ -166,13 +167,6 @@ size_t b200_dcn_enqueue_workspace_size(const b200_tensor_desc *in, const int32_t
                                  padding[0], dilation[1], dilation[0]);
 }
 
-// Output extent of one spatial axis; 0 for a geometry with no output.
-static long long dcn_out_extent(long long in, long long k, long long s, long long p, long long d) {
-  if (in <= 0 || k <= 0 || s <= 0 || p < 0 || d <= 0) return 0;
-  const long long n = in + 2 * p - (d * (k - 1) + 1);
-  return n < 0 ? 0 : n / s + 1;
-}
-
 static bool dims_are(const b200_dims &d, long long d0, long long d1, long long d2, long long d3) {
   return d.nbDims == 4 && d.d[0] == d0 && d.d[1] == d1 && d.d[2] == d2 && d.d[3] == d3;
 }
@@ -183,9 +177,15 @@ static bool dcn_geometry_ok(const b200_tensor_desc *in, const b200_tensor_desc *
                             int pw, int dh, int dw, int groups, int deform_groups) {
   const b200_dims &x = in[0].dims, &w = in[3].dims;
   if (x.nbDims != 4 || w.nbDims != 4 || groups <= 0 || deform_groups <= 0) return false;
-  const long long n = x.d[0], c = x.d[1], co = w.d[0], kh = w.d[2], kw = w.d[3], taps = kh * kw;
-  const long long ho = dcn_out_extent(x.d[2], kh, sh, ph, dh), wo = dcn_out_extent(x.d[3], kw, sw, pw, dw);
-  if (n <= 0 || ho <= 0 || wo <= 0 || static_cast<long long>(w.d[1]) * groups != c) return false;
+  const long long n = x.d[0], c = x.d[1], h = x.d[2], wd = x.d[3], co = w.d[0], kh = w.d[2], kw = w.d[3], taps = kh * kw;
+  if (n <= 0 || h <= 0 || wd <= 0 || kh <= 0 || kw <= 0 || sh <= 0 || sw <= 0 || dh <= 0 || dw <= 0) return false;
+  // Beyond the launchers' rule: TensorRT floors the output extent, so the dilated kernel must fit the padded input (a
+  // numerator in (-stride, 0) truncates to a 1-pixel output), and padding is never negative.
+  if (ph < 0 || pw < 0 || dcn_extent_numerator<long long>(h, kh, ph, dh) < 0 ||
+      dcn_extent_numerator<long long>(wd, kw, pw, dw) < 0)
+    return false;
+  const long long ho = dcn_out_extent<long long>(h, kh, sh, ph, dh), wo = dcn_out_extent<long long>(wd, kw, sw, pw, dw);
+  if (static_cast<long long>(w.d[1]) * groups != c) return false;
   if (nb_inputs == 5 && !(in[4].dims.nbDims == 1 && in[4].dims.d[0] == co)) return false;
   return dims_are(in[1].dims, n, deform_groups * 2 * taps, ho, wo) && dims_are(in[2].dims, n, deform_groups * taps, ho, wo) &&
          dims_are(out[0].dims, n, co, ho, wo);

@@ -15,31 +15,9 @@
 #include <cstdlib>
 #include <type_traits>
 
-#include "common.cuh"
+#include "dcn_geometry.cuh"
 
 namespace b200 {
-
-// dcn_fused.cu
-size_t dcn_fused_workspace_bytes(int batch, int channels, int height, int width, int channels_out, int kk);
-bool dcn_fused_supported(int channels, int channels_out, int kk, int group, int deformable_group);
-int dcn_fused_f16(const __half *input, const __half *weight, const __half *bias, const __half *offset,
-                  const __half *mask, __half *output, void *workspace, int batch, int channels, int height, int width,
-                  int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h,
-                  int dilation_w, int dilation_h, int Ho, int Wo, int flags, cudaStream_t stream);
-int dcn_pack_weights_f16(const __half *weight, __half *packed, int channels_out, int channels, int kk, cudaStream_t stream);
-
-int dcn_fused_i8(const int8_t *input, float scale_i, const int8_t *weight, float scale_w, const void *bias, int bias_is_half,
-                 const int8_t *offset, float scale_off, const int8_t *mask, float scale_mask, int8_t *output, float scale_o,
-                 void *workspace, int batch, int channels, int height, int width, int channels_out, int kernel_w,
-                 int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w, int dilation_h, int Ho,
-                 int Wo, cudaStream_t stream);
-
-// dcn_generic.cu
-template <typename T>
-int dcn_generic_launch(const T *input, const T *weight, const T *bias, const T *offset, const T *mask, T *output, int batch,
-                       int channels, int height, int width, int channels_out, int kernel_w, int kernel_h, int stride_w,
-                       int stride_h, int pad_w, int pad_h, int dilation_w, int dilation_h, int group, int deformable_group,
-                       int Ho, int Wo, cudaStream_t stream);
 
 // -1: read B200_DCN_FUSED once (default on). Atomic: enqueue may run on several host threads (SURVEY §8(b)).
 static std::atomic<int> g_dcn_fused{-1};
@@ -55,38 +33,26 @@ static bool dcn_fused_enabled() {
 
 template <typename T>
 static int dcn_forward(const T *input, const T *weight, const T *bias, const T *offset, const T *mask, T *output,
-                       void *workspace, int batch, int channels, int height, int width, int channels_out, int kernel_w,
-                       int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w, int dilation_h,
-                       int group, int deformable_group, cudaStream_t stream) {
+                       void *workspace, const DcnGeom &g, cudaStream_t stream) {
   if (!input || !weight || !offset || !mask || !output) return B200_ERR_BAD_PARAM;
-  if (batch <= 0 || channels <= 0 || height <= 0 || width <= 0 || channels_out <= 0 || kernel_w <= 0 ||
-      kernel_h <= 0 || stride_w <= 0 || stride_h <= 0 || dilation_w <= 0 || dilation_h <= 0 || group <= 0 ||
-      deformable_group <= 0)
-    return B200_ERR_BAD_PARAM;
+  if (!dcn_positive(g)) return B200_ERR_BAD_PARAM;
   // the reference exit(1)s on these (…Conv2dPlugin.cpp:300-336); here they are a status
-  if (channels % group || channels_out % group || channels % deformable_group) return B200_ERR_UNSUPPORTED;
-  const int Ho = (height + 2 * pad_h - (dilation_h * (kernel_h - 1) + 1)) / stride_h + 1;
-  const int Wo = (width + 2 * pad_w - (dilation_w * (kernel_w - 1) + 1)) / stride_w + 1;
-  if (Ho <= 0 || Wo <= 0) return B200_ERR_BAD_PARAM;
-  const long long HoWo = static_cast<long long>(Ho) * Wo;
-  const int kk = kernel_h * kernel_w;
-  if (static_cast<long long>(channels) * kk * HoWo >= (1ll << 31)) return B200_ERR_BAD_PARAM;
+  if (!dcn_groups_divide(g)) return B200_ERR_UNSUPPORTED;
+  if (g.Ho <= 0 || g.Wo <= 0) return B200_ERR_BAD_PARAM;
+  if (static_cast<long long>(g.C) * (g.kh * g.kw) * (static_cast<long long>(g.Ho) * g.Wo) >= (1ll << 31))
+    return B200_ERR_BAD_PARAM;
 
   // the fused pre-passes use 128-bit accesses: unaligned views (storage offsets) take the generic kernel instead
   const bool aligned = workspace && reinterpret_cast<uintptr_t>(workspace) % 256 == 0 &&
                        reinterpret_cast<uintptr_t>(input) % 16 == 0 && reinterpret_cast<uintptr_t>(weight) % 16 == 0 &&
                        reinterpret_cast<uintptr_t>(output) % 16 == 0;
   // the wgmma kernel reads FP16 bits: BF16 (also 2 bytes) takes the generic kernel
-  if (std::is_same<T, __half>::value && aligned && dcn_fused_enabled() &&
-      dcn_fused_supported(channels, channels_out, kk, group, deformable_group))
+  if (std::is_same<T, __half>::value && aligned && dcn_fused_enabled() && dcn_fused_supported(g))
     return dcn_fused_f16(reinterpret_cast<const __half *>(input), reinterpret_cast<const __half *>(weight),
                          reinterpret_cast<const __half *>(bias), reinterpret_cast<const __half *>(offset),
-                         reinterpret_cast<const __half *>(mask), reinterpret_cast<__half *>(output), workspace, batch,
-                         channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w, pad_h,
-                         dilation_w, dilation_h, Ho, Wo, 0, stream);
-  return dcn_generic_launch<T>(input, weight, bias, offset, mask, output, batch, channels, height, width, channels_out,
-                               kernel_w, kernel_h, stride_w, stride_h, pad_w, pad_h, dilation_w, dilation_h, group,
-                               deformable_group, Ho, Wo, stream);
+                         reinterpret_cast<const __half *>(mask), reinterpret_cast<__half *>(output), workspace, g, 0,
+                         stream);
+  return dcn_generic_launch<T>(input, weight, bias, offset, mask, output, g, stream);
 }
 
 // ---- INT8 for the shapes the fused tensor-core kernel does not take (groups / deformable groups > 1, other channel
@@ -119,56 +85,47 @@ __global__ void dcn_f16_to_i8_kernel(const __half *in, float inv_scale, int8_t *
     out[i] = static_cast<int8_t>(to_int8_sat(__half2float(in[i]) * inv_scale));
 }
 
-static size_t align256(size_t b) { return (b + 255) / 256 * 256; }
-
 struct DcnI8Plan {  // byte offsets into the workspace
-  size_t x, w, off, mask, bias, out, col, total;
+  size_t x, w, off, mask, bias, out, total;
 };
-static DcnI8Plan dcn_i8_plan(int batch, int channels, int height, int width, int channels_out, int kh, int kw, int Ho,
-                             int Wo, int group, int dg) {
+static DcnI8Plan dcn_i8_plan(const DcnGeom &g) {
   DcnI8Plan p{};
   size_t o = 0;
-  p.x = o, o += align256(static_cast<size_t>(batch) * channels * height * width * 2);
-  p.w = o, o += align256(static_cast<size_t>(channels_out) * (channels / group) * kh * kw * 2);
-  p.off = o, o += align256(static_cast<size_t>(batch) * dg * 2 * kh * kw * Ho * Wo * 2);
-  p.mask = o, o += align256(static_cast<size_t>(batch) * dg * kh * kw * Ho * Wo * 2);
-  p.bias = o, o += align256(static_cast<size_t>(channels_out) * 2);
-  p.out = o, o += align256(static_cast<size_t>(batch) * channels_out * Ho * Wo * 2);
-  p.col = o;  // (no column buffer: the generic kernel samples straight into shared memory)
-  p.total = o;
+  p.x = o, o += align256(static_cast<size_t>(g.B) * g.C * g.H * g.W * 2);
+  p.w = o, o += align256(static_cast<size_t>(g.Co) * (g.C / g.groups) * g.kh * g.kw * 2);
+  p.off = o, o += align256(static_cast<size_t>(g.B) * g.dg * 2 * g.kh * g.kw * g.Ho * g.Wo * 2);
+  p.mask = o, o += align256(static_cast<size_t>(g.B) * g.dg * g.kh * g.kw * g.Ho * g.Wo * 2);
+  p.bias = o, o += align256(static_cast<size_t>(g.Co) * 2);
+  p.out = o, o += align256(static_cast<size_t>(g.B) * g.Co * g.Ho * g.Wo * 2);
+  p.total = o;  // (no column buffer: the generic kernel samples straight into shared memory)
   return p;
 }
 
-static unsigned grid_for(long long n) { return static_cast<unsigned>(n / 256 + 1 < (1 << 20) ? n / 256 + 1 : (1 << 20)); }
-
 static int dcn_i8_unfused(const int8_t *input, float scale_i, const int8_t *weight, float scale_w, const void *bias,
                           int bias_is_half, const int8_t *offset, float scale_off, const int8_t *mask, float scale_mask,
-                          int8_t *output, float scale_o, void *workspace, int batch, int channels, int height, int width,
-                          int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h,
-                          int dilation_w, int dilation_h, int Ho, int Wo, int group, int dg, cudaStream_t s) {
-  if (group <= 0 || dg <= 0) return B200_ERR_BAD_PARAM;
-  if (channels % 4 || (channels / group) % 4 || channels % group || channels_out % group || channels % dg)
+                          int8_t *output, float scale_o, void *workspace, const DcnGeom &g, cudaStream_t s) {
+  if (g.groups <= 0 || g.dg <= 0) return B200_ERR_BAD_PARAM;
+  if (g.C % 4 || (g.C / g.groups) % 4 || !dcn_groups_divide(g))
     return B200_ERR_UNSUPPORTED;  // kCHW4 packs 4 channels; the reference exit(1)s on the group mismatches
-  const DcnI8Plan pl = dcn_i8_plan(batch, channels, height, width, channels_out, kernel_h, kernel_w, Ho, Wo, group, dg);
+  const DcnI8Plan pl = dcn_i8_plan(g);
   char *ws = static_cast<char *>(workspace);
   __half *x = reinterpret_cast<__half *>(ws + pl.x), *w = reinterpret_cast<__half *>(ws + pl.w);
   __half *off = reinterpret_cast<__half *>(ws + pl.off), *msk = reinterpret_cast<__half *>(ws + pl.mask);
   __half *b = reinterpret_cast<__half *>(ws + pl.bias), *out = reinterpret_cast<__half *>(ws + pl.out);
-  const long long plane = static_cast<long long>(height) * width, kk = static_cast<long long>(kernel_h) * kernel_w;
-  const long long nx = static_cast<long long>(batch) * (channels / 4) * plane;
-  const long long nw = static_cast<long long>(channels_out) * (channels / group / 4) * kk;
-  const long long noff = static_cast<long long>(batch) * dg * 2 * kk * Ho * Wo, nout = static_cast<long long>(batch) * channels_out * Ho * Wo;
-  dcn_i8_chw4_to_nchw_f16_kernel<<<grid_for(nx), 256, 0, s>>>(input, scale_i, x, channels, plane, nx);
-  dcn_i8_chw4_to_nchw_f16_kernel<<<grid_for(nw), 256, 0, s>>>(weight, scale_w, w, channels / group, kk, nw);
+  const long long plane = static_cast<long long>(g.H) * g.W, kk = static_cast<long long>(g.kh) * g.kw;
+  const long long nx = static_cast<long long>(g.B) * (g.C / 4) * plane;
+  const long long nw = static_cast<long long>(g.Co) * (g.C / g.groups / 4) * kk;
+  const long long noff = static_cast<long long>(g.B) * g.dg * 2 * kk * g.Ho * g.Wo;
+  const long long nout = static_cast<long long>(g.B) * g.Co * g.Ho * g.Wo;
+  dcn_i8_chw4_to_nchw_f16_kernel<<<grid_for(nx), 256, 0, s>>>(input, scale_i, x, g.C, plane, nx);
+  dcn_i8_chw4_to_nchw_f16_kernel<<<grid_for(nw), 256, 0, s>>>(weight, scale_w, w, g.C / g.groups, kk, nw);
   dcn_i8_to_f16_kernel<<<grid_for(noff), 256, 0, s>>>(offset, scale_off, off, noff);
   dcn_i8_to_f16_kernel<<<grid_for(noff / 2), 256, 0, s>>>(mask, scale_mask, msk, noff / 2);
-  if (bias) dcn_bias_to_f16_kernel<<<(channels_out + 255) / 256, 256, 0, s>>>(bias, bias_is_half, b, channels_out);
+  if (bias) dcn_bias_to_f16_kernel<<<(g.Co + 255) / 256, 256, 0, s>>>(bias, bias_is_half, b, g.Co);
   g_launch_count.fetch_add(bias ? 4 : 3, std::memory_order_relaxed);
   int st = check_launch();
   if (st != B200_OK) return st;
-  st = dcn_forward<__half>(x, w, bias ? b : nullptr, off, msk, out, nullptr, batch, channels, height, width,
-                           channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w, pad_h, dilation_w, dilation_h,
-                           group, dg, s);
+  st = dcn_forward<__half>(x, w, bias ? b : nullptr, off, msk, out, nullptr, g, s);
   if (st != B200_OK) return st;
   dcn_f16_to_i8_kernel<<<grid_for(nout), 256, 0, s>>>(out, 1.f / scale_o, output, nout);
   return check_launch();
@@ -192,16 +149,31 @@ __global__ void dcn_chw2_to_nchw_kernel(const __half2 *in, __half *out, int C, l
 struct DcnChw2Plan {
   size_t x, off, w, rest, total;
 };
-static DcnChw2Plan dcn_chw2_plan(int batch, int channels, int height, int width, int channels_out, int kh, int kw, int Ho,
-                                 int Wo, int group, int dg, size_t inner) {
+static DcnChw2Plan dcn_chw2_plan(const DcnGeom &g, size_t inner) {
   DcnChw2Plan p{};
   size_t o = 0;
-  p.x = o, o += align256(static_cast<size_t>(batch) * channels * height * width * 2);
-  p.off = o, o += align256(static_cast<size_t>(batch) * dg * 2 * kh * kw * Ho * Wo * 2);
-  p.w = o, o += align256(static_cast<size_t>(channels_out) * (channels / group) * kh * kw * 2);
+  p.x = o, o += align256(static_cast<size_t>(g.B) * g.C * g.H * g.W * 2);
+  p.off = o, o += align256(static_cast<size_t>(g.B) * g.dg * 2 * g.kh * g.kw * g.Ho * g.Wo * 2);
+  p.w = o, o += align256(static_cast<size_t>(g.Co) * (g.C / g.groups) * g.kh * g.kw * 2);
   p.rest = o, o += inner;
   p.total = o;
   return p;
+}
+
+// The layers a workspace query sizes (it returns 0 for any other). Looser than the launchers' check: the kernel size,
+// the dilation and the input's height and width are looked at only through Ho and Wo.
+static bool dcn_query_ok(const DcnGeom &g) {
+  return g.stride_h > 0 && g.stride_w > 0 && g.groups > 0 && g.dg > 0 && g.Ho > 0 && g.Wo > 0 && g.B > 0 && g.C > 0 &&
+         g.Co > 0;
+}
+
+// b200_dcn_workspace_size(1, ...): the fused FP16 kernel's workspace for the largest channels_out it takes (the query
+// has no channels_out argument, nor has the reference's formula). The generic kernel needs none (the reference sizes a
+// column buffer here, …Conv2dPlugin.cpp:73-115). Never 0: hosts pass a real pointer.
+static size_t dcn_f16_workspace_bytes(DcnGeom g) {
+  g.Co = 512;
+  const size_t fused = dcn_fused_workspace_bytes(g);
+  return fused > 256 ? fused : 256;
 }
 
 }  // namespace b200
@@ -212,29 +184,19 @@ extern "C" {
 
 size_t b200_dcn_workspace_size(int dtype, int batch, int channels, int height, int width, int kernel_w, int kernel_h,
                                int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w, int dilation_h) {
-  if (stride_h <= 0 || stride_w <= 0) return 0;
-  const int Ho = (height + 2 * pad_h - (dilation_h * (kernel_h - 1) + 1)) / stride_h + 1;
-  const int Wo = (width + 2 * pad_w - (dilation_w * (kernel_w - 1) + 1)) / stride_w + 1;
-  if (Ho <= 0 || Wo <= 0 || batch <= 0 || channels <= 0) return 0;
-  // The generic kernel needs no workspace (the reference sizes a column buffer here, …Conv2dPlugin.cpp:73-115). The
-  // fused FP16 path needs the NHWC copy of the input + the permuted weights (channels_out is not an argument of the
-  // reference's formula either; 512 is the largest the fused path takes). FP32 (0) and BF16 (7) run the generic kernel
-  // only. Never 0: hosts pass a real pointer.
-  const size_t fused = dtype == 0 || dtype == 7 ? 0 : dcn_fused_workspace_bytes(batch, channels, height, width, 512, kernel_h * kernel_w);
-  return fused > 256 ? fused : 256;
+  const DcnGeom g = dcn_geom(batch, channels, height, width, 512, kernel_w, kernel_h, stride_w, stride_h, pad_w, pad_h,
+                             dilation_w, dilation_h, 1, 1);
+  if (!dcn_query_ok(g)) return 0;
+  return dtype == 0 || dtype == 7 ? 256 : dcn_f16_workspace_bytes(g);  // FP32 and BF16 run the generic kernel only
 }
 
 size_t b200_dcn_i8_workspace_size(int batch, int channels, int height, int width, int channels_out, int kernel_w,
                                   int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
                                   int dilation_h, int group, int deformable_group) {
-  if (stride_h <= 0 || stride_w <= 0 || group <= 0 || deformable_group <= 0) return 0;
-  const int Ho = (height + 2 * pad_h - (dilation_h * (kernel_h - 1) + 1)) / stride_h + 1;
-  const int Wo = (width + 2 * pad_w - (dilation_w * (kernel_w - 1) + 1)) / stride_w + 1;
-  if (Ho <= 0 || Wo <= 0 || batch <= 0 || channels <= 0 || channels_out <= 0) return 0;
-  const size_t fused = b200_dcn_workspace_size(1, batch, channels, height, width, kernel_w, kernel_h, stride_w, stride_h,
-                                               pad_w, pad_h, dilation_w, dilation_h);
-  const size_t unfused = dcn_i8_plan(batch, channels, height, width, channels_out, kernel_h, kernel_w, Ho, Wo, group,
-                                     deformable_group).total;
+  const DcnGeom g = dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
+                             pad_h, dilation_w, dilation_h, group, deformable_group);
+  if (!dcn_query_ok(g)) return 0;
+  const size_t fused = dcn_f16_workspace_bytes(g), unfused = dcn_i8_plan(g).total;
   return fused > unfused ? fused : unfused;
 }
 
@@ -247,155 +209,135 @@ int b200_dcn_set_fused(int enabled) {  // enabled < 0: query only
 int b200_dcn_pack_weights_f16(const void *weight, void *packed, int channels_out, int channels, int kernel_h, int kernel_w,
                               void *stream) {
   if (!weight || !packed || channels_out <= 0 || channels <= 0 || kernel_h <= 0 || kernel_w <= 0) return B200_ERR_BAD_PARAM;
-  if (!dcn_fused_supported(channels, channels_out, kernel_h * kernel_w, 1, 1)) return B200_ERR_UNSUPPORTED;
-  return dcn_pack_weights_f16(static_cast<const __half *>(weight), static_cast<__half *>(packed), channels_out, channels,
-                              kernel_h * kernel_w, static_cast<cudaStream_t>(stream));
+  DcnGeom g{};  // packing depends on the weight's shape alone
+  g.C = channels, g.Co = channels_out, g.kh = kernel_h, g.kw = kernel_w, g.groups = g.dg = 1;
+  if (!dcn_fused_supported(g)) return B200_ERR_UNSUPPORTED;
+  return dcn_pack_weights_f16(static_cast<const __half *>(weight), static_cast<__half *>(packed), g,
+                              static_cast<cudaStream_t>(stream));
 }
 
 int b200_dcn_f16_ex(const void *input, const void *weight, const void *bias, const void *offset, const void *mask,
                     void *output, void *workspace, int batch, int channels, int height, int width, int channels_out,
                     int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
                     int dilation_h, int group, int deformable_group, int flags, void *stream) {
+  const DcnGeom g = dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
+                             pad_h, dilation_w, dilation_h, group, deformable_group);
   if (!input || !weight || !offset || !mask || !output || !workspace) return B200_ERR_BAD_PARAM;
-  if (batch <= 0 || channels <= 0 || height <= 0 || width <= 0 || channels_out <= 0 || kernel_w <= 0 || kernel_h <= 0 ||
-      stride_w <= 0 || stride_h <= 0 || dilation_w <= 0 || dilation_h <= 0)
-    return B200_ERR_BAD_PARAM;
-  const int Ho = (height + 2 * pad_h - (dilation_h * (kernel_h - 1) + 1)) / stride_h + 1;
-  const int Wo = (width + 2 * pad_w - (dilation_w * (kernel_w - 1) + 1)) / stride_w + 1;
-  if (Ho <= 0 || Wo <= 0) return B200_ERR_BAD_PARAM;
-  if (!dcn_fused_supported(channels, channels_out, kernel_h * kernel_w, group, deformable_group) ||
-      reinterpret_cast<uintptr_t>(workspace) % 256 != 0 || reinterpret_cast<uintptr_t>(input) % 16 != 0 ||
-      reinterpret_cast<uintptr_t>(weight) % 16 != 0)
+  if (!dcn_positive(g) || g.Ho <= 0 || g.Wo <= 0) return B200_ERR_BAD_PARAM;
+  if (!dcn_fused_supported(g) || reinterpret_cast<uintptr_t>(workspace) % 256 != 0 ||
+      reinterpret_cast<uintptr_t>(input) % 16 != 0 || reinterpret_cast<uintptr_t>(weight) % 16 != 0)
     return B200_ERR_UNSUPPORTED;
   return dcn_fused_f16(static_cast<const __half *>(input), static_cast<const __half *>(weight),
                        static_cast<const __half *>(bias), static_cast<const __half *>(offset),
-                       static_cast<const __half *>(mask), static_cast<__half *>(output), workspace, batch, channels,
-                       height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w, pad_h, dilation_w,
-                       dilation_h, Ho, Wo, flags, static_cast<cudaStream_t>(stream));
+                       static_cast<const __half *>(mask), static_cast<__half *>(output), workspace, g, flags,
+                       static_cast<cudaStream_t>(stream));
 }
 
 int b200_dcn_i8(const int8_t *input, float scale_i, const int8_t *weight, float scale_w, const void *bias, int bias_is_half,
                 const int8_t *offset, float scale_off, const int8_t *mask, float scale_mask, int8_t *output, float scale_o,
                 void *workspace, int batch, int channels, int height, int width, int channels_out, int kernel_w,
                 int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w, int dilation_h, int group,
-                int deformable_group, int im2col_step, void *cublas_handle, void *stream) {
-  (void)im2col_step;
-  (void)cublas_handle;
+                int deformable_group, int /*im2col_step*/, void * /*cublas_handle*/, void *stream) {
+  const DcnGeom g = dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
+                             pad_h, dilation_w, dilation_h, group, deformable_group);
   if (!input || !weight || !offset || !mask || !output || !workspace) return B200_ERR_BAD_PARAM;
-  if (batch <= 0 || channels <= 0 || height <= 0 || width <= 0 || channels_out <= 0 || kernel_w <= 0 || kernel_h <= 0 ||
-      stride_w <= 0 || stride_h <= 0 || dilation_w <= 0 || dilation_h <= 0 || !(scale_o > 0.f))
-    return B200_ERR_BAD_PARAM;
-  const int Ho = (height + 2 * pad_h - (dilation_h * (kernel_h - 1) + 1)) / stride_h + 1;
-  const int Wo = (width + 2 * pad_w - (dilation_w * (kernel_w - 1) + 1)) / stride_w + 1;
-  if (Ho <= 0 || Wo <= 0) return B200_ERR_BAD_PARAM;
+  // the group counts are checked on the unfused path, after the alignment checks
+  if (!dcn_extents_positive(g) || !(scale_o > 0.f) || g.Ho <= 0 || g.Wo <= 0) return B200_ERR_BAD_PARAM;
   if (reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return B200_ERR_UNSUPPORTED;
   // both pre-passes read the kCHW4 input (and the unfused one the weight) as 32-bit packets
   if (reinterpret_cast<uintptr_t>(input) % 4 != 0 || reinterpret_cast<uintptr_t>(weight) % 4 != 0)
     return B200_ERR_UNSUPPORTED;
   // every DCN of the BEVFormer backbones takes the fused tensor-core path; other shapes dequantise into the workspace
   // (sized by b200_dcn_i8_workspace_size) and run the generic fused kernel
-  if (!dcn_fused_enabled() || !dcn_fused_supported(channels, channels_out, kernel_h * kernel_w, group, deformable_group))
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!dcn_fused_enabled() || !dcn_fused_supported(g))
     return dcn_i8_unfused(input, scale_i, weight, scale_w, bias, bias_is_half, offset, scale_off, mask, scale_mask,
-                          output, scale_o, workspace, batch, channels, height, width, channels_out, kernel_w, kernel_h,
-                          stride_w, stride_h, pad_w, pad_h, dilation_w, dilation_h, Ho, Wo, group, deformable_group,
-                          static_cast<cudaStream_t>(stream));
+                          output, scale_o, workspace, g, s);
   return dcn_fused_i8(input, scale_i, weight, scale_w, bias, bias_is_half, offset, scale_off, mask, scale_mask, output,
-                      scale_o, workspace, batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w,
-                      stride_h, pad_w, pad_h, dilation_w, dilation_h, Ho, Wo, static_cast<cudaStream_t>(stream));
+                      scale_o, workspace, g, s);
 }
 
+// im2col_step is ignored: the reference computes it but loops per image anyway (…Kernel.cu:711-735).
 int b200_dcn_f32(const float *input, const float *weight, const float *bias, const float *offset, const float *mask,
                  float *output, void *workspace, int batch, int channels, int height, int width, int channels_out,
                  int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
-                 int dilation_h, int group, int deformable_group, int im2col_step, void *cublas_handle, void *stream) {
-  (void)im2col_step;  // the reference computes it but loops per image anyway (…Kernel.cu:711-735)
-  (void)cublas_handle;
-  return dcn_forward<float>(input, weight, bias, offset, mask, output, workspace, batch, channels, height, width,
-                            channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w, pad_h, dilation_w, dilation_h,
-                            group, deformable_group, static_cast<cudaStream_t>(stream));
+                 int dilation_h, int group, int deformable_group, int /*im2col_step*/, void * /*cublas_handle*/,
+                 void *stream) {
+  return dcn_forward<float>(input, weight, bias, offset, mask, output, workspace,
+                            dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h,
+                                     pad_w, pad_h, dilation_w, dilation_h, group, deformable_group),
+                            static_cast<cudaStream_t>(stream));
 }
 
 int b200_dcn_f16(const void *input, const void *weight, const void *bias, const void *offset, const void *mask,
                  void *output, void *workspace, int batch, int channels, int height, int width, int channels_out,
                  int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
-                 int dilation_h, int group, int deformable_group, int im2col_step, void *cublas_handle, void *stream) {
-  (void)im2col_step;
-  (void)cublas_handle;
-  return dcn_forward<__half>(static_cast<const __half *>(input), static_cast<const __half *>(weight),
-                             static_cast<const __half *>(bias), static_cast<const __half *>(offset),
-                             static_cast<const __half *>(mask), static_cast<__half *>(output), workspace, batch,
-                             channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
-                             pad_h, dilation_w, dilation_h, group, deformable_group,
-                             static_cast<cudaStream_t>(stream));
+                 int dilation_h, int group, int deformable_group, int /*im2col_step*/, void * /*cublas_handle*/,
+                 void *stream) {
+  using H = __half;
+  return dcn_forward<H>(static_cast<const H *>(input), static_cast<const H *>(weight), static_cast<const H *>(bias),
+                        static_cast<const H *>(offset), static_cast<const H *>(mask), static_cast<H *>(output),
+                        workspace,
+                        dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h,
+                                 pad_w, pad_h, dilation_w, dilation_h, group, deformable_group),
+                        static_cast<cudaStream_t>(stream));
 }
 
 // BF16: the generic kernel (fp32 accumulation, one rounding per output); there is no BF16 tensor-core path.
 int b200_dcn_bf16(const void *input, const void *weight, const void *bias, const void *offset, const void *mask,
                   void *output, void *workspace, int batch, int channels, int height, int width, int channels_out,
                   int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
-                  int dilation_h, int group, int deformable_group, int im2col_step, void *cublas_handle, void *stream) {
-  (void)im2col_step;
-  (void)cublas_handle;
+                  int dilation_h, int group, int deformable_group, int /*im2col_step*/, void * /*cublas_handle*/,
+                  void *stream) {
   using B = __nv_bfloat16;
   return dcn_forward<B>(static_cast<const B *>(input), static_cast<const B *>(weight), static_cast<const B *>(bias),
                         static_cast<const B *>(offset), static_cast<const B *>(mask), static_cast<B *>(output),
-                        workspace, batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h,
-                        pad_w, pad_h, dilation_w, dilation_h, group, deformable_group,
+                        workspace,
+                        dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h,
+                                 pad_w, pad_h, dilation_w, dilation_h, group, deformable_group),
                         static_cast<cudaStream_t>(stream));
 }
 
 size_t b200_dcn_f16_chw2_workspace_size(int batch, int channels, int height, int width, int channels_out, int kernel_w,
                                         int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
                                         int dilation_h, int group, int deformable_group) {
-  if (stride_h <= 0 || stride_w <= 0 || group <= 0 || deformable_group <= 0) return 0;
-  const int Ho = (height + 2 * pad_h - (dilation_h * (kernel_h - 1) + 1)) / stride_h + 1;
-  const int Wo = (width + 2 * pad_w - (dilation_w * (kernel_w - 1) + 1)) / stride_w + 1;
-  if (Ho <= 0 || Wo <= 0 || batch <= 0 || channels <= 0 || channels_out <= 0) return 0;
-  const size_t inner = b200_dcn_workspace_size(1, batch, channels, height, width, kernel_w, kernel_h, stride_w, stride_h,
-                                               pad_w, pad_h, dilation_w, dilation_h);
-  return dcn_chw2_plan(batch, channels, height, width, channels_out, kernel_h, kernel_w, Ho, Wo, group, deformable_group,
-                       inner).total;
+  const DcnGeom g = dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
+                             pad_h, dilation_w, dilation_h, group, deformable_group);
+  if (!dcn_query_ok(g)) return 0;
+  return dcn_chw2_plan(g, dcn_f16_workspace_bytes(g)).total;
 }
 
 int b200_dcn_f16_chw2(const void *input, const void *weight, const void *bias, const void *offset, const void *mask,
                       void *output, void *workspace, int batch, int channels, int height, int width, int channels_out,
                       int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w,
-                      int dilation_h, int group, int deformable_group, int im2col_step, void *cublas_handle, void *stream) {
-  (void)im2col_step;
-  (void)cublas_handle;
+                      int dilation_h, int group, int deformable_group, int /*im2col_step*/, void * /*cublas_handle*/,
+                      void *stream) {
+  const DcnGeom g = dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
+                             pad_h, dilation_w, dilation_h, group, deformable_group);
   if (!input || !weight || !offset || !mask || !output || !workspace) return B200_ERR_BAD_PARAM;
-  if (batch <= 0 || channels <= 0 || height <= 0 || width <= 0 || channels_out <= 0 || kernel_w <= 0 || kernel_h <= 0 ||
-      stride_w <= 0 || stride_h <= 0 || dilation_w <= 0 || dilation_h <= 0 || group <= 0 || deformable_group <= 0)
-    return B200_ERR_BAD_PARAM;
-  if (channels % group || channels_out % group || channels % deformable_group) return B200_ERR_UNSUPPORTED;
+  if (!dcn_positive(g)) return B200_ERR_BAD_PARAM;
+  if (!dcn_groups_divide(g)) return B200_ERR_UNSUPPORTED;
   if (reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return B200_ERR_UNSUPPORTED;
-  const int Ho = (height + 2 * pad_h - (dilation_h * (kernel_h - 1) + 1)) / stride_h + 1;
-  const int Wo = (width + 2 * pad_w - (dilation_w * (kernel_w - 1) + 1)) / stride_w + 1;
-  if (Ho <= 0 || Wo <= 0) return B200_ERR_BAD_PARAM;
-  const size_t inner = b200_dcn_workspace_size(1, batch, channels, height, width, kernel_w, kernel_h, stride_w, stride_h,
-                                               pad_w, pad_h, dilation_w, dilation_h);
-  const DcnChw2Plan pl = dcn_chw2_plan(batch, channels, height, width, channels_out, kernel_h, kernel_w, Ho, Wo, group,
-                                       deformable_group, inner);
+  if (g.Ho <= 0 || g.Wo <= 0) return B200_ERR_BAD_PARAM;
+  const DcnChw2Plan pl = dcn_chw2_plan(g, dcn_f16_workspace_bytes(g));
   char *ws = static_cast<char *>(workspace);
   __half *x = reinterpret_cast<__half *>(ws + pl.x), *off = reinterpret_cast<__half *>(ws + pl.off);
   __half *w = reinterpret_cast<__half *>(ws + pl.w);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const long long plane = static_cast<long long>(height) * width, kk = static_cast<long long>(kernel_h) * kernel_w;
-  const int coff = deformable_group * 2 * static_cast<int>(kk), cw = channels / group;
-  const long long nx = static_cast<long long>(batch) * ((channels + 1) / 2) * plane;
-  const long long no = static_cast<long long>(batch) * ((coff + 1) / 2) * Ho * Wo;
-  const long long nw = static_cast<long long>(channels_out) * ((cw + 1) / 2) * kk;
-  dcn_chw2_to_nchw_kernel<<<grid_for(nx), 256, 0, s>>>(static_cast<const __half2 *>(input), x, channels, plane, nx);
+  const long long plane = static_cast<long long>(g.H) * g.W, kk = static_cast<long long>(g.kh) * g.kw;
+  const int coff = g.dg * 2 * static_cast<int>(kk), cw = g.C / g.groups;
+  const long long nx = static_cast<long long>(g.B) * ((g.C + 1) / 2) * plane;
+  const long long no = static_cast<long long>(g.B) * ((coff + 1) / 2) * g.Ho * g.Wo;
+  const long long nw = static_cast<long long>(g.Co) * ((cw + 1) / 2) * kk;
+  dcn_chw2_to_nchw_kernel<<<grid_for(nx), 256, 0, s>>>(static_cast<const __half2 *>(input), x, g.C, plane, nx);
   dcn_chw2_to_nchw_kernel<<<grid_for(no), 256, 0, s>>>(static_cast<const __half2 *>(offset), off, coff,
-                                                      static_cast<long long>(Ho) * Wo, no);
+                                                      static_cast<long long>(g.Ho) * g.Wo, no);
   dcn_chw2_to_nchw_kernel<<<grid_for(nw), 256, 0, s>>>(static_cast<const __half2 *>(weight), w, cw, kk, nw);
   g_launch_count.fetch_add(2, std::memory_order_relaxed);
   const int st = check_launch();
   if (st != B200_OK) return st;
   return dcn_forward<__half>(x, w, static_cast<const __half *>(bias), off, static_cast<const __half *>(mask),
-                             static_cast<__half *>(output), ws + pl.rest, batch, channels, height, width, channels_out,
-                             kernel_w, kernel_h, stride_w, stride_h, pad_w, pad_h, dilation_w, dilation_h, group,
-                             deformable_group, s);
+                             static_cast<__half *>(output), ws + pl.rest, g, s);
 }
 
 }  // extern "C"

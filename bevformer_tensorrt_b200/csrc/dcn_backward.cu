@@ -25,12 +25,9 @@
 #include <algorithm>
 #include <type_traits>
 
-#include "common.cuh"
+#include "dcn_geometry.cuh"
 
 namespace b200 {
-
-bool dcn_fused_supported(int channels, int channels_out, int kk, int group, int deformable_group);  // dcn_fused.cu
-
 namespace {
 
 constexpr int kBT = 64;      // pixels per tile
@@ -419,12 +416,9 @@ __global__ void dcn_bw_f32_round_kernel(const float *in, T *out, long long n) {
     bw_st(out + i, in[i]);
 }
 
-unsigned grid_for(long long n) { return static_cast<unsigned>(n / 256 + 1 < (1 << 20) ? n / 256 + 1 : (1 << 20)); }
-size_t align256(size_t b) { return (b + 255) / 256 * 256; }
-
 // Everything the launches need that follows from the geometry alone (also what the workspace query returns).
 struct BwPlan {
-  int Ho, Wo, kk, KC, npass, nsplit, wsplit;
+  int KC, npass, nsplit, wsplit;
   size_t gin, om, w, total;  // byte offsets of the workspace sections
   size_t smem_data, smem_weight;
 };
@@ -436,37 +430,28 @@ int pick_kc_bw(int Cg, int cpd, int kk) {
 }
 
 // 0 on success, else the status to return
-int bw_plan(BwPlan &pl, int f16, int batch, int channels, int height, int width, int channels_out, int kernel_w,
-            int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w, int dilation_h, int group,
-            int deformable_group) {
-  if (batch <= 0 || channels <= 0 || height <= 0 || width <= 0 || channels_out <= 0 || kernel_w <= 0 || kernel_h <= 0 ||
-      stride_w <= 0 || stride_h <= 0 || dilation_w <= 0 || dilation_h <= 0 || pad_w < 0 || pad_h < 0 || group <= 0 ||
-      deformable_group <= 0)
+int bw_plan(BwPlan &pl, bool f16, const DcnGeom &g) {
+  if (!dcn_positive(g) || g.pad_h < 0 || g.pad_w < 0 || !dcn_groups_divide(g) || g.Ho <= 0 || g.Wo <= 0)
     return B200_ERR_BAD_PARAM;
-  if (channels % group || channels_out % group || channels % deformable_group) return B200_ERR_BAD_PARAM;
-  pl.Ho = (height + 2 * pad_h - (dilation_h * (kernel_h - 1) + 1)) / stride_h + 1;
-  pl.Wo = (width + 2 * pad_w - (dilation_w * (kernel_w - 1) + 1)) / stride_w + 1;
-  if (pl.Ho <= 0 || pl.Wo <= 0) return B200_ERR_BAD_PARAM;
-  const long long P = static_cast<long long>(pl.Ho) * pl.Wo, kk = static_cast<long long>(kernel_h) * kernel_w;
+  const long long P = static_cast<long long>(g.Ho) * g.Wo, kk = static_cast<long long>(g.kh) * g.kw;
   // 32-bit offsets inside planes and tiles; every tensor below 2^31 elements
-  if (static_cast<long long>(channels) * kk * P >= (1ll << 31) || static_cast<long long>(batch) * channels * height * width >= (1ll << 31) ||
-      static_cast<long long>(batch) * channels_out * P >= (1ll << 31) || static_cast<long long>(batch) * deformable_group * 2 * kk * P >= (1ll << 31))
+  if (static_cast<long long>(g.C) * kk * P >= (1ll << 31) || static_cast<long long>(g.B) * g.C * g.H * g.W >= (1ll << 31) ||
+      static_cast<long long>(g.B) * g.Co * P >= (1ll << 31) || static_cast<long long>(g.B) * g.dg * 2 * kk * P >= (1ll << 31))
     return B200_ERR_BAD_PARAM;
-  pl.kk = static_cast<int>(kk);
-  const int Cg = channels / group, cpd = channels / deformable_group, Mg = channels_out / group;
-  pl.KC = pick_kc_bw(Cg, cpd, pl.kk);
-  pl.npass = pl.KC > 1 ? 1 : (pl.kk + kRB - 1) / kRB;
+  const int Cg = g.C / g.groups, cpd = g.C / g.dg, Mg = g.Co / g.groups;
+  pl.KC = pick_kc_bw(Cg, cpd, static_cast<int>(kk));
+  pl.npass = pl.KC > 1 ? 1 : (static_cast<int>(kk) + kRB - 1) / kRB;
   const int ptiles = static_cast<int>((P + kBT - 1) / kBT);
   const int nch = cpd / pl.KC;
-  pl.nsplit = std::min(nch, std::max(1, (kTargetCtas + deformable_group * ptiles - 1) / (deformable_group * ptiles)));
-  const long long wbase = static_cast<long long>((Mg + 63) / 64) * group * (Cg / pl.KC) * pl.npass;
-  const long long items = static_cast<long long>(batch) * ptiles;
+  pl.nsplit = std::min(nch, std::max(1, (kTargetCtas + g.dg * ptiles - 1) / (g.dg * ptiles)));
+  const long long wbase = static_cast<long long>((Mg + 63) / 64) * g.groups * (Cg / pl.KC) * pl.npass;
+  const long long items = static_cast<long long>(g.B) * ptiles;
   pl.wsplit = static_cast<int>(std::min<long long>(items, std::max<long long>(1, (4 * kTargetCtas + wbase - 1) / wbase)));
   if (wbase > 65535) return B200_ERR_UNSUPPORTED;
   size_t o = 0;
-  pl.gin = o, o += f16 ? align256(static_cast<size_t>(batch) * channels * height * width * 4) : 0;
-  pl.om = o, o += align256(static_cast<size_t>(batch) * deformable_group * pl.nsplit * 3 * kk * P * 4);
-  pl.w = o, o += align256(static_cast<size_t>(pl.wsplit) * channels_out * Cg * kk * 4);
+  pl.gin = o, o += f16 ? align256(static_cast<size_t>(g.B) * g.C * g.H * g.W * 4) : 0;
+  pl.om = o, o += align256(static_cast<size_t>(g.B) * g.dg * pl.nsplit * 3 * kk * P * 4);
+  pl.w = o, o += align256(static_cast<size_t>(pl.wsplit) * g.Co * Cg * kk * 4);
   pl.total = o;
   pl.smem_data = (kMC * kBT + kMC * kRB + 3 * kRB * kBT + 3 * kk * kBT) * 4 + kk * kBT * sizeof(BwTap);
   pl.smem_weight = (kBT * kLdA + kBT * kLdB) * 4 + std::min<long long>(kk, kRB) * kBT * sizeof(BwTap);
@@ -476,16 +461,13 @@ int bw_plan(BwPlan &pl, int f16, int batch, int channels, int height, int width,
 
 template <typename T>
 int dcn_backward(const T *input, const T *weight, const T *offset, const T *mask, const T *grad_output, T *grad_input,
-                 T *grad_weight, T *grad_bias, T *grad_offset, T *grad_mask, void *workspace, int batch, int channels,
-                 int height, int width, int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h,
-                 int pad_w, int pad_h, int dilation_w, int dilation_h, int group, int deformable_group, int flags,
+                 T *grad_weight, T *grad_bias, T *grad_offset, T *grad_mask, void *workspace, const DcnGeom &g, int flags,
                  cudaStream_t s) {
   constexpr bool kF16 = sizeof(T) == 2;  // FP16 or BF16: grad_input is accumulated in the fp32 workspace
   if (!input || !weight || !offset || !mask || !grad_output || !workspace) return B200_ERR_BAD_PARAM;
   if (flags & ~3) return B200_ERR_BAD_PARAM;
   BwPlan pl{};
-  int st = bw_plan(pl, kF16, batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
-                   pad_h, dilation_w, dilation_h, group, deformable_group);
+  int st = bw_plan(pl, kF16, g);
   if (st != B200_OK) return st;
   const void *ptrs[] = {input, weight, offset, mask, grad_output, grad_input, grad_weight, grad_bias, grad_offset, grad_mask};
   for (const void *q : ptrs)
@@ -493,19 +475,19 @@ int dcn_backward(const T *input, const T *weight, const T *offset, const T *mask
   if (reinterpret_cast<uintptr_t>(workspace) % 256) return B200_ERR_BAD_PARAM;
   if (flags) {  // the layouts of b200_dcn_f16_ex: its envelope and alignment
     if (reinterpret_cast<uintptr_t>(input) % 16 || reinterpret_cast<uintptr_t>(weight) % 16) return B200_ERR_BAD_PARAM;
-    if (!std::is_same<T, __half>::value || !dcn_fused_supported(channels, channels_out, pl.kk, group, deformable_group)) return B200_ERR_UNSUPPORTED;
+    if (!std::is_same<T, __half>::value || !dcn_fused_supported(g)) return B200_ERR_UNSUPPORTED;
   }
   if (!grad_input && !grad_weight && !grad_bias && !grad_offset && !grad_mask) return B200_OK;
 
   char *ws = static_cast<char *>(workspace);
-  const long long HW = static_cast<long long>(height) * width, P = static_cast<long long>(pl.Ho) * pl.Wo;
-  const long long nx = static_cast<long long>(batch) * channels * HW;
+  const int kk = g.kh * g.kw;
+  const long long HW = static_cast<long long>(g.H) * g.W, P = static_cast<long long>(g.Ho) * g.Wo;
+  const long long nx = static_cast<long long>(g.B) * g.C * HW;
 
   DcnBwParams p{};
   p.im = input, p.weight = weight, p.offset = offset, p.mask = mask, p.gout = grad_output;
-  p.B = batch, p.C = channels, p.H = height, p.W = width, p.Co = channels_out, p.kh = kernel_h, p.kw = kernel_w;
-  p.pad_h = pad_h, p.pad_w = pad_w, p.stride_h = stride_h, p.stride_w = stride_w, p.dil_h = dilation_h, p.dil_w = dilation_w;
-  p.groups = group, p.dg = deformable_group, p.Ho = pl.Ho, p.Wo = pl.Wo;
+  dcn_set_layer(p, g);
+  p.groups = g.groups, p.dg = g.dg;
   p.KC = pl.KC, p.npass = pl.npass, p.nsplit = pl.nsplit, p.wsplit = pl.wsplit;
   p.nhwc = flags & 1, p.packed = (flags >> 1) & 1;
   const unsigned ptiles = static_cast<unsigned>((P + kBT - 1) / kBT);
@@ -517,8 +499,8 @@ int dcn_backward(const T *input, const T *weight, const T *offset, const T *mask
     if (cudaFuncSetAttribute(dcn_bw_data_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              static_cast<int>(pl.smem_data)) != cudaSuccess)
       return B200_ERR_LAUNCH;
-    if (static_cast<long long>(deformable_group) * pl.nsplit > 65535 || batch > 65535) return B200_ERR_UNSUPPORTED;
-    dcn_bw_data_kernel<T><<<dim3(ptiles, deformable_group * pl.nsplit, batch), kThreads, pl.smem_data, s>>>(p);
+    if (static_cast<long long>(g.dg) * pl.nsplit > 65535 || g.B > 65535) return B200_ERR_UNSUPPORTED;
+    dcn_bw_data_kernel<T><<<dim3(ptiles, g.dg * pl.nsplit, g.B), kThreads, pl.smem_data, s>>>(p);
     if ((st = check_launch()) != B200_OK) return st;
     if constexpr (kF16) {
       if (grad_input) {
@@ -527,29 +509,28 @@ int dcn_backward(const T *input, const T *weight, const T *offset, const T *mask
       }
     }
     if (p.om_part) {
-      const long long n = static_cast<long long>(batch) * deformable_group * pl.kk * P;
-      dcn_bw_sum_offset_mask_kernel<T><<<grid_for(n), 256, 0, s>>>(p.om_part, grad_offset, grad_mask,
-                                                                  batch * deformable_group, pl.kk, static_cast<int>(P),
-                                                                  pl.nsplit);
+      const long long n = static_cast<long long>(g.B) * g.dg * kk * P;
+      dcn_bw_sum_offset_mask_kernel<T><<<grid_for(n), 256, 0, s>>>(p.om_part, grad_offset, grad_mask, g.B * g.dg, kk,
+                                                                  static_cast<int>(P), pl.nsplit);
       if ((st = check_launch()) != B200_OK) return st;
     }
   }
   if (grad_weight) {
     p.gin = nullptr, p.om_part = nullptr, p.w_part = reinterpret_cast<float *>(ws + pl.w);
-    const int Cg = channels / group, Mg = channels_out / group;
-    const dim3 grid((Mg + 63) / 64, group * (Cg / pl.KC) * pl.npass, pl.wsplit);
+    const int Cg = g.C / g.groups, Mg = g.Co / g.groups;
+    const dim3 grid((Mg + 63) / 64, g.groups * (Cg / pl.KC) * pl.npass, pl.wsplit);
     if (grid.y > 65535u || grid.z > 65535u) return B200_ERR_UNSUPPORTED;
     if (cudaFuncSetAttribute(dcn_bw_weight_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              static_cast<int>(pl.smem_weight)) != cudaSuccess)
       return B200_ERR_LAUNCH;
     dcn_bw_weight_kernel<T><<<grid, kThreads, pl.smem_weight, s>>>(p);
     if ((st = check_launch()) != B200_OK) return st;
-    const long long n = static_cast<long long>(channels_out) * Cg * pl.kk;
+    const long long n = static_cast<long long>(g.Co) * Cg * kk;
     dcn_bw_sum_weight_kernel<T><<<grid_for(n), 256, 0, s>>>(p.w_part, grad_weight, n, pl.wsplit);
     if ((st = check_launch()) != B200_OK) return st;
   }
   if (grad_bias) {
-    dcn_bw_bias_kernel<T><<<channels_out, kThreads, 0, s>>>(grad_output, grad_bias, batch, channels_out, static_cast<int>(P));
+    dcn_bw_bias_kernel<T><<<g.Co, kThreads, 0, s>>>(grad_output, grad_bias, g.B, g.Co, static_cast<int>(P));
     if ((st = check_launch()) != B200_OK) return st;
   }
   return B200_OK;
@@ -566,8 +547,8 @@ size_t b200_dcn_backward_workspace_size(int dtype, int batch, int channels, int 
                                         int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h,
                                         int dilation_w, int dilation_h, int group, int deformable_group) {
   BwPlan pl{};
-  if (bw_plan(pl, dtype != 0, batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
-              pad_h, dilation_w, dilation_h, group, deformable_group) != B200_OK)
+  if (bw_plan(pl, dtype != 0, dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w,
+                                       stride_h, pad_w, pad_h, dilation_w, dilation_h, group, deformable_group)) != B200_OK)
     return 0;
   return pl.total;
 }
@@ -578,9 +559,10 @@ int b200_dcn_backward_f32(const float *input, const float *weight, const float *
                           int width, int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w,
                           int pad_h, int dilation_w, int dilation_h, int group, int deformable_group, void *stream) {
   return dcn_backward<float>(input, weight, offset, mask, grad_output, grad_input, grad_weight, grad_bias, grad_offset,
-                             grad_mask, workspace, batch, channels, height, width, channels_out, kernel_w, kernel_h,
-                             stride_w, stride_h, pad_w, pad_h, dilation_w, dilation_h, group, deformable_group, 0,
-                             static_cast<cudaStream_t>(stream));
+                             grad_mask, workspace,
+                             dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w,
+                                      stride_h, pad_w, pad_h, dilation_w, dilation_h, group, deformable_group),
+                             0, static_cast<cudaStream_t>(stream));
 }
 
 int b200_dcn_backward_f16(const void *input, const void *weight, const void *offset, const void *mask,
@@ -589,14 +571,14 @@ int b200_dcn_backward_f16(const void *input, const void *weight, const void *off
                           int width, int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w,
                           int pad_h, int dilation_w, int dilation_h, int group, int deformable_group, int flags,
                           void *stream) {
-  return dcn_backward<__half>(static_cast<const __half *>(input), static_cast<const __half *>(weight),
-                              static_cast<const __half *>(offset), static_cast<const __half *>(mask),
-                              static_cast<const __half *>(grad_output), static_cast<__half *>(grad_input),
-                              static_cast<__half *>(grad_weight), static_cast<__half *>(grad_bias),
-                              static_cast<__half *>(grad_offset), static_cast<__half *>(grad_mask), workspace, batch,
-                              channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h, pad_w,
-                              pad_h, dilation_w, dilation_h, group, deformable_group, flags,
-                              static_cast<cudaStream_t>(stream));
+  using H = __half;
+  return dcn_backward<H>(static_cast<const H *>(input), static_cast<const H *>(weight), static_cast<const H *>(offset),
+                         static_cast<const H *>(mask), static_cast<const H *>(grad_output), static_cast<H *>(grad_input),
+                         static_cast<H *>(grad_weight), static_cast<H *>(grad_bias), static_cast<H *>(grad_offset),
+                         static_cast<H *>(grad_mask), workspace,
+                         dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h,
+                                  pad_w, pad_h, dilation_w, dilation_h, group, deformable_group),
+                         flags, static_cast<cudaStream_t>(stream));
 }
 
 // BF16: every tensor and gradient in bf16, fp32 accumulation; no flags (there is no BF16 fused forward whose layouts
@@ -610,9 +592,10 @@ int b200_dcn_backward_bf16(const void *input, const void *weight, const void *of
   return dcn_backward<B>(static_cast<const B *>(input), static_cast<const B *>(weight), static_cast<const B *>(offset),
                          static_cast<const B *>(mask), static_cast<const B *>(grad_output), static_cast<B *>(grad_input),
                          static_cast<B *>(grad_weight), static_cast<B *>(grad_bias), static_cast<B *>(grad_offset),
-                         static_cast<B *>(grad_mask), workspace, batch, channels, height, width, channels_out, kernel_w,
-                         kernel_h, stride_w, stride_h, pad_w, pad_h, dilation_w, dilation_h, group, deformable_group, 0,
-                         static_cast<cudaStream_t>(stream));
+                         static_cast<B *>(grad_mask), workspace,
+                         dcn_geom(batch, channels, height, width, channels_out, kernel_w, kernel_h, stride_w, stride_h,
+                                  pad_w, pad_h, dilation_w, dilation_h, group, deformable_group),
+                         0, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

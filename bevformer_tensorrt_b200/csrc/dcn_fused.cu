@@ -25,7 +25,7 @@
 // C % 64 == 0, Co in {128, 256, 512}, kh*kw <= 9.
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint)
 
-#include "common.cuh"
+#include "dcn_geometry.cuh"
 
 namespace b200 {
 
@@ -434,16 +434,27 @@ __global__ void __launch_bounds__(kFusedThreads, 1) dcn_fused_kernel(const DcnFu
 }
 
 // ---- host -----------------------------------------------------------------------------------------------------------
-size_t dcn_fused_workspace_bytes(int batch, int channels, int height, int width, int channels_out, int kk) {
-  const size_t x = (static_cast<size_t>(batch) * height * width * channels * 2 + 255) / 256 * 256;
-  const size_t w = (static_cast<size_t>(channels_out) * channels * kk * 2 + 255) / 256 * 256;
-  return x + w + 2048;  // + a zero / fp32 bias vector (<= 512 channels x 4 B)
+bool dcn_fused_supported(const DcnGeom &g) {
+  return g.groups == 1 && g.dg == 1 && g.C % kBK == 0 && (g.Co == 128 || g.Co == 256 || g.Co == 512) &&
+         g.kh * g.kw <= kMaxTaps;
 }
 
-bool dcn_fused_supported(int channels, int channels_out, int kk, int group, int deformable_group) {
-  return group == 1 && deformable_group == 1 && channels % kBK == 0 &&
-         (channels_out == 128 || channels_out == 256 || channels_out == 512) && kk <= kMaxTaps;
+// Byte offsets of the workspace sections: the NHWC copy of the input, the permuted weights, and the bias vector the
+// epilogue reads (FP16 zeros when there is no bias, or the INT8 flavour's fp32 bias), with room for 512 fp32 values:
+// the largest Co the kernel takes.
+struct DcnFusedLayout {
+  size_t x, w, bias, total;
+};
+static DcnFusedLayout dcn_fused_layout(const DcnGeom &g) {
+  DcnFusedLayout l{};
+  size_t o = 0;
+  l.x = o, o += align256(static_cast<size_t>(g.B) * g.H * g.W * g.C * 2);
+  l.w = o, o += align256(static_cast<size_t>(g.Co) * g.C * (g.kh * g.kw) * 2);
+  l.bias = o, o += 512 * sizeof(float);
+  l.total = o;
+  return l;
 }
+size_t dcn_fused_workspace_bytes(const DcnGeom &g) { return dcn_fused_layout(g).total; }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
@@ -470,7 +481,7 @@ static int make_weight_tmap(CUtensorMap *tm, const __half *w_r, int Co, int K) {
 }
 
 template <int MH, bool I8>
-static int launch_fused(const DcnFusedParams &p, cudaStream_t stream) {
+static int launch_fused_mh(const DcnFusedParams &p, cudaStream_t stream) {
   using Cfg = FusedCfg<MH>;
   // per launch: the attribute is per device (and this may run on several devices / host threads); the call is cheap
   if (cudaFuncSetAttribute(dcn_fused_kernel<MH, I8>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes) !=
@@ -487,62 +498,62 @@ static int launch_fused(const DcnFusedParams &p, cudaStream_t stream) {
   return check_launch();
 }
 
+// The layer, its k-block and tile counts into `p` (whose tensors are set), then the launch for Co = 128 * MH.
+template <bool I8>
+static int launch_fused(DcnFusedParams &p, const DcnGeom &g, cudaStream_t stream) {
+  dcn_set_layer(p, g);
+  p.kb_per_tap = g.C / kBK;
+  p.num_kb = g.kh * g.kw * p.kb_per_tap;
+  const int mh = g.Co / 128;
+  const int bn = mh == 1 ? FusedCfg<1>::kBN : (mh == 2 ? FusedCfg<2>::kBN : FusedCfg<4>::kBN);
+  p.tiles_per_img = (g.Ho * g.Wo + bn - 1) / bn;
+  p.num_tiles = p.tiles_per_img * g.B;
+  switch (mh) {
+    case 1: return launch_fused_mh<1, I8>(p, stream);
+    case 2: return launch_fused_mh<2, I8>(p, stream);
+    case 4: return launch_fused_mh<4, I8>(p, stream);
+    default: return B200_ERR_UNSUPPORTED;
+  }
+}
+
 int dcn_fused_f16(const __half *input, const __half *weight, const __half *bias, const __half *offset,
-                  const __half *mask, __half *output, void *workspace, int batch, int channels, int height, int width,
-                  int channels_out, int kernel_w, int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h,
-                  int dilation_w, int dilation_h, int Ho, int Wo, int flags, cudaStream_t stream) {
+                  const __half *mask, __half *output, void *workspace, const DcnGeom &g, int flags, cudaStream_t stream) {
   // flags: bit 0 = `input` is already NHWC (channels-last), bit 1 = `weight` is already permuted (b200_dcn_pack_weights_f16)
-  const int kk = kernel_h * kernel_w, HW = height * width;
-  __half *x_nhwc = static_cast<__half *>(workspace);
-  __half *w_r = reinterpret_cast<__half *>(static_cast<uint8_t *>(workspace) +
-                                           (static_cast<size_t>(batch) * HW * channels * 2 + 255) / 256 * 256);
+  const int kk = g.kh * g.kw, HW = g.H * g.W;
+  const DcnFusedLayout l = dcn_fused_layout(g);
+  uint8_t *ws = static_cast<uint8_t *>(workspace);
+  __half *x_nhwc = reinterpret_cast<__half *>(ws + l.x), *w_r = reinterpret_cast<__half *>(ws + l.w);
   if (!bias) {  // the kernel always reads a bias vector (no per-thread null test in the epilogue): use zeros
-    __half *zb = reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(w_r) +
-                                            (static_cast<size_t>(channels_out) * channels * kk * 2 + 255) / 256 * 256);
-    if (cudaMemsetAsync(zb, 0, static_cast<size_t>(channels_out) * 2, stream) != cudaSuccess) return B200_ERR_LAUNCH;
+    __half *zb = reinterpret_cast<__half *>(ws + l.bias);
+    if (cudaMemsetAsync(zb, 0, static_cast<size_t>(g.Co) * 2, stream) != cudaSuccess) return B200_ERR_LAUNCH;
     bias = zb;
   }
   int st = B200_OK;
   if (flags & 1) {
     x_nhwc = const_cast<__half *>(input);
   } else {
-    dcn_nchw_to_nhwc_kernel<<<dim3((HW + 63) / 64, channels / 64, batch), 512, 0, stream>>>(input, x_nhwc, channels, HW);
+    dcn_nchw_to_nhwc_kernel<<<dim3((HW + 63) / 64, g.C / 64, g.B), 512, 0, stream>>>(input, x_nhwc, g.C, HW);
     st = check_launch();
     if (st != B200_OK) return st;
   }
   if (flags & 2) {
     w_r = const_cast<__half *>(weight);
   } else {
-    const long long wn = static_cast<long long>(channels_out) * channels * kk;
-    dcn_weight_reorder_kernel<<<static_cast<unsigned>((wn + 255) / 256), 256, 0, stream>>>(weight, w_r, channels_out,
-                                                                                           channels, kk);
+    const long long wn = static_cast<long long>(g.Co) * g.C * kk;
+    dcn_weight_reorder_kernel<<<static_cast<unsigned>((wn + 255) / 256), 256, 0, stream>>>(weight, w_r, g.Co, g.C, kk);
     st = check_launch();
     if (st != B200_OK) return st;
   }
 
   DcnFusedParams p{};
   p.x_nhwc = x_nhwc, p.w_r = w_r, p.bias = bias, p.offset = offset, p.mask = mask, p.out = output;
-  p.B = batch, p.C = channels, p.H = height, p.W = width, p.Co = channels_out, p.kh = kernel_h, p.kw = kernel_w;
-  p.pad_h = pad_h, p.pad_w = pad_w, p.stride_h = stride_h, p.stride_w = stride_w, p.dil_h = dilation_h,
-  p.dil_w = dilation_w, p.Ho = Ho, p.Wo = Wo;
-  p.kb_per_tap = channels / kBK;
-  p.num_kb = kk * p.kb_per_tap;
-  const int mh = channels_out / 128;
-  const int bn = mh == 1 ? FusedCfg<1>::kBN : (mh == 2 ? FusedCfg<2>::kBN : FusedCfg<4>::kBN);
-  p.tiles_per_img = (Ho * Wo + bn - 1) / bn;
-  p.num_tiles = p.tiles_per_img * batch;
-  switch (mh) {
-    case 1: return launch_fused<1, false>(p, stream);
-    case 2: return launch_fused<2, false>(p, stream);
-    case 4: return launch_fused<4, false>(p, stream);
-    default: return B200_ERR_UNSUPPORTED;
-  }
+  return launch_fused<false>(p, g, stream);
 }
 
-int dcn_pack_weights_f16(const __half *weight, __half *packed, int channels_out, int channels, int kk, cudaStream_t stream) {
-  const long long wn = static_cast<long long>(channels_out) * channels * kk;
-  dcn_weight_reorder_kernel<<<static_cast<unsigned>((wn + 255) / 256), 256, 0, stream>>>(weight, packed, channels_out,
-                                                                                         channels, kk);
+int dcn_pack_weights_f16(const __half *weight, __half *packed, const DcnGeom &g, cudaStream_t stream) {
+  const int kk = g.kh * g.kw;
+  const long long wn = static_cast<long long>(g.Co) * g.C * kk;
+  dcn_weight_reorder_kernel<<<static_cast<unsigned>((wn + 255) / 256), 256, 0, stream>>>(weight, packed, g.Co, g.C, kk);
   return check_launch();
 }
 
@@ -601,47 +612,28 @@ __global__ void dcn_bias_to_f32_kernel(const void *bias, int is_half, float *out
 
 int dcn_fused_i8(const int8_t *input, float scale_i, const int8_t *weight, float scale_w, const void *bias, int bias_is_half,
                  const int8_t *offset, float scale_off, const int8_t *mask, float scale_mask, int8_t *output, float scale_o,
-                 void *workspace, int batch, int channels, int height, int width, int channels_out, int kernel_w,
-                 int kernel_h, int stride_w, int stride_h, int pad_w, int pad_h, int dilation_w, int dilation_h, int Ho,
-                 int Wo, cudaStream_t stream) {
-  const int kk = kernel_h * kernel_w, HW = height * width;
+                 void *workspace, const DcnGeom &g, cudaStream_t stream) {
+  const int kk = g.kh * g.kw, HW = g.H * g.W;
+  const DcnFusedLayout l = dcn_fused_layout(g);
   uint8_t *ws = static_cast<uint8_t *>(workspace);
-  __half *x_nhwc = reinterpret_cast<__half *>(ws);
-  ws += (static_cast<size_t>(batch) * HW * channels * 2 + 255) / 256 * 256;
-  __half *w_r = reinterpret_cast<__half *>(ws);
-  ws += (static_cast<size_t>(channels_out) * channels * kk * 2 + 255) / 256 * 256;
-  float *bias_f = reinterpret_cast<float *>(ws);  // 512 floats fit the 2 KB tail reserved by dcn_fused_workspace_bytes
+  __half *x_nhwc = reinterpret_cast<__half *>(ws + l.x), *w_r = reinterpret_cast<__half *>(ws + l.w);
+  float *bias_f = reinterpret_cast<float *>(ws + l.bias);
 
-  dcn_chw4_to_nhwc_f16_kernel<<<dim3((HW + 63) / 64, channels / 64, batch), 256, 0, stream>>>(input, x_nhwc, channels, HW);
+  dcn_chw4_to_nhwc_f16_kernel<<<dim3((HW + 63) / 64, g.C / 64, g.B), 256, 0, stream>>>(input, x_nhwc, g.C, HW);
   int st = check_launch();
   if (st != B200_OK) return st;
-  const long long wn = static_cast<long long>(channels_out) * channels * kk;
-  dcn_weight_reorder_i8_kernel<<<static_cast<unsigned>((wn + 255) / 256), 256, 0, stream>>>(weight, w_r, channels_out,
-                                                                                            channels, kk);
+  const long long wn = static_cast<long long>(g.Co) * g.C * kk;
+  dcn_weight_reorder_i8_kernel<<<static_cast<unsigned>((wn + 255) / 256), 256, 0, stream>>>(weight, w_r, g.Co, g.C, kk);
   st = check_launch();
   if (st != B200_OK) return st;
-  dcn_bias_to_f32_kernel<<<(channels_out + 255) / 256, 256, 0, stream>>>(bias, bias_is_half, bias_f, channels_out);
+  dcn_bias_to_f32_kernel<<<(g.Co + 255) / 256, 256, 0, stream>>>(bias, bias_is_half, bias_f, g.Co);
   st = check_launch();
   if (st != B200_OK) return st;
 
   DcnFusedParams p{};
   p.x_nhwc = x_nhwc, p.w_r = w_r, p.bias = bias_f, p.offset = offset, p.mask = mask, p.out = output;
   p.scale_off = scale_off, p.scale_mask = scale_mask, p.out_mul = scale_i * scale_w, p.out_div = scale_o, p.out_inv = 1.f / scale_o;
-  p.B = batch, p.C = channels, p.H = height, p.W = width, p.Co = channels_out, p.kh = kernel_h, p.kw = kernel_w;
-  p.pad_h = pad_h, p.pad_w = pad_w, p.stride_h = stride_h, p.stride_w = stride_w, p.dil_h = dilation_h,
-  p.dil_w = dilation_w, p.Ho = Ho, p.Wo = Wo;
-  p.kb_per_tap = channels / kBK;
-  p.num_kb = kk * p.kb_per_tap;
-  const int mh = channels_out / 128;
-  const int bn = mh == 1 ? FusedCfg<1>::kBN : (mh == 2 ? FusedCfg<2>::kBN : FusedCfg<4>::kBN);
-  p.tiles_per_img = (Ho * Wo + bn - 1) / bn;
-  p.num_tiles = p.tiles_per_img * batch;
-  switch (mh) {
-    case 1: return launch_fused<1, true>(p, stream);
-    case 2: return launch_fused<2, true>(p, stream);
-    case 4: return launch_fused<4, true>(p, stream);
-    default: return B200_ERR_UNSUPPORTED;
-  }
+  return launch_fused<true>(p, g, stream);
 }
 
 }  // namespace b200

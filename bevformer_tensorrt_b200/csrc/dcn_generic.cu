@@ -17,7 +17,7 @@
 //   * the B tile (KC*kk x 64 pixels) is sampled straight into shared memory through that table (consecutive threads =
 //     consecutive pixels), the A tile (64 x KC*kk weights) is read k-contiguous and stored transposed;
 //   * fp32 FMAs from shared memory, bias added in the epilogue, FP16 / BF16 storage converted at load / store only.
-#include "common.cuh"
+#include "dcn_geometry.cuh"
 
 namespace b200 {
 
@@ -182,24 +182,21 @@ static int pick_kc(int Cg, int cpd, int kk) {
 }
 
 template <typename T>
-int dcn_generic_launch(const T *input, const T *weight, const T *bias, const T *offset, const T *mask, T *output, int batch,
-                       int channels, int height, int width, int channels_out, int kernel_w, int kernel_h, int stride_w,
-                       int stride_h, int pad_w, int pad_h, int dilation_w, int dilation_h, int group, int deformable_group,
-                       int Ho, int Wo, cudaStream_t stream) {
+int dcn_generic_launch(const T *input, const T *weight, const T *bias, const T *offset, const T *mask, T *output,
+                       const DcnGeom &g, cudaStream_t stream) {
   DcnGParams p{};
   p.im = input, p.weight = weight, p.bias = bias, p.offset = offset, p.mask = mask, p.out = output;
-  p.B = batch, p.C = channels, p.H = height, p.W = width, p.Co = channels_out, p.kh = kernel_h, p.kw = kernel_w;
-  p.pad_h = pad_h, p.pad_w = pad_w, p.stride_h = stride_h, p.stride_w = stride_w, p.dil_h = dilation_h, p.dil_w = dilation_w;
-  p.groups = group, p.dg = deformable_group, p.Ho = Ho, p.Wo = Wo;
-  const int kk = kernel_h * kernel_w, Cg = channels / group, cpd = channels / deformable_group;
+  dcn_set_layer(p, g);
+  p.groups = g.groups, p.dg = g.dg;
+  const int kk = g.kh * g.kw, Cg = g.C / g.groups, cpd = g.C / g.dg;
   p.KC = pick_kc(Cg, cpd, kk);
   const int KB = p.KC * kk;
   const size_t smem = static_cast<size_t>(KB) * (kGT + 1) * 4 + 16 + static_cast<size_t>(KB) * kGT * 4 +
                       static_cast<size_t>(kk) * kGT * sizeof(DcnTap);
   if (smem > 200 * 1024) return B200_ERR_UNSUPPORTED;  // kernels beyond ~12x12 taps
-  const long long HoWo = static_cast<long long>(Ho) * Wo;
-  const dim3 grid(static_cast<unsigned>((HoWo + kGT - 1) / kGT), static_cast<unsigned>((channels_out / group + kGT - 1) / kGT),
-                  static_cast<unsigned>(batch * group));
+  const long long HoWo = static_cast<long long>(g.Ho) * g.Wo;
+  const dim3 grid(static_cast<unsigned>((HoWo + kGT - 1) / kGT), static_cast<unsigned>((g.Co / g.groups + kGT - 1) / kGT),
+                  static_cast<unsigned>(g.B * g.groups));
   if (grid.y > 65535u || grid.z > 65535u) return B200_ERR_UNSUPPORTED;
   if (cudaFuncSetAttribute(dcn_generic_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)) !=
       cudaSuccess)
@@ -208,15 +205,8 @@ int dcn_generic_launch(const T *input, const T *weight, const T *bias, const T *
   return check_launch();
 }
 
-template int dcn_generic_launch<float>(const float *, const float *, const float *, const float *, const float *, float *,
-                                       int, int, int, int, int, int, int, int, int, int, int, int, int, int, int, int, int,
-                                       cudaStream_t);
-template int dcn_generic_launch<__half>(const __half *, const __half *, const __half *, const __half *, const __half *,
-                                        __half *, int, int, int, int, int, int, int, int, int, int, int, int, int, int, int,
-                                        int, int, cudaStream_t);
-template int dcn_generic_launch<__nv_bfloat16>(const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *,
-                                               const __nv_bfloat16 *, const __nv_bfloat16 *, __nv_bfloat16 *, int, int,
-                                               int, int, int, int, int, int, int, int, int, int, int, int, int, int, int,
-                                               cudaStream_t);
+template int dcn_generic_launch(const float *, const float *, const float *, const float *, const float *, float *, const DcnGeom &, cudaStream_t);
+template int dcn_generic_launch(const __half *, const __half *, const __half *, const __half *, const __half *, __half *, const DcnGeom &, cudaStream_t);
+template int dcn_generic_launch(const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, const __nv_bfloat16 *, __nv_bfloat16 *, const DcnGeom &, cudaStream_t);
 
 }  // namespace b200
