@@ -2,10 +2,18 @@
 // enqueue / supportsFormatCombination mirrors for MSDA (reference: multiScaleDeformableAttnPlugin.cpp:71-189).
 #include "common.cuh"
 #include "dcn_geometry.cuh"
+#include "msda_geometry.cuh"
 
 namespace b200 {
 std::atomic<unsigned long long> g_launch_count{0};
+
+// Shape unpacking of the reference's MSDA plugin (…Plugin.cpp:75-88): batch / spatial / heads / channels from value's
+// dims, L = `levels` (shapes.d[0]), G from ref.d[3] / 2, Q from offsets.d[1], P from weights.d[3] / L.
+static MsdaGeom msda_desc_geom(const b200_tensor_desc *in, int levels) {
+  const int32_t *v = in[0].dims.d;
+  return msda_geom(v[0], v[1], v[2], v[3], levels, in[3].dims.d[1], in[4].dims.d[3] / levels, in[2].dims.d[3] / 2);
 }
+}  // namespace b200
 
 using namespace b200;
 
@@ -25,44 +33,41 @@ const char *b200_status_string(int status) {
 
 unsigned long long b200_launch_count(void) { return g_launch_count.load(std::memory_order_relaxed); }
 
-// IPluginV2DynamicExt::enqueue of the reference, argument for argument (…Plugin.cpp:71-140). Shape unpacking is the
-// reference's: batch/spatial/heads/channels from value dims, L from shapes.d[0], G from ref.d[3]/2, Q from
-// offsets.d[1], P from weights.d[3]/L; scales from the tensor descriptors (:75-88).
+// IPluginV2DynamicExt::enqueue of the reference, argument for argument (…Plugin.cpp:71-140), with msda_desc_geom's
+// shapes and the scales of the tensor descriptors.
 int b200_msda_enqueue(const b200_tensor_desc *in, const b200_tensor_desc *out, const void *const *inputs,
                       void *const *outputs, void *workspace, void *stream, int use_h2) {
   // The reference asks for 0 workspace bytes (…Plugin.cpp:64-69). A host that lends b200_msda_enqueue_workspace_size()
   // bytes gets the second-generation INT8 kernels (msda_v2.cu); workspace == NULL keeps the round-1 kernels.
   if (!in || !out || !inputs || !outputs) return B200_ERR_BAD_PARAM;
-  const int batch = in[0].dims.d[0], spatial = in[0].dims.d[1], heads = in[0].dims.d[2], ch = in[0].dims.d[3];
-  const int levels = in[1].dims.d[0];
-  if (levels <= 0) return B200_ERR_BAD_PARAM;
-  const int G = in[2].dims.d[3] / 2, Q = in[3].dims.d[1], P = in[4].dims.d[3] / levels;
+  if (in[1].dims.d[0] <= 0) return B200_ERR_BAD_PARAM;
+  const MsdaGeom g = msda_desc_geom(in, in[1].dims.d[0]);
   const int32_t *shapes = static_cast<const int32_t *>(inputs[1]);
   switch (in[0].type) {
     case 0:  // kFLOAT
       return b200_msda_f32(static_cast<const float *>(inputs[0]), shapes, static_cast<const float *>(inputs[2]),
-                           static_cast<const float *>(inputs[3]), static_cast<const float *>(inputs[4]), batch,
-                           spatial, heads, ch, levels, Q, P, G, static_cast<float *>(outputs[0]), stream);
+                           static_cast<const float *>(inputs[3]), static_cast<const float *>(inputs[4]), g.B, g.S, g.M,
+                           g.C, g.L, g.Q, g.P, g.G, static_cast<float *>(outputs[0]), stream);
     case 1:  // kHALF
-      if (use_h2 && ch % 2 == 0)
-        return b200_msda_f16_h2(inputs[0], shapes, inputs[2], inputs[3], inputs[4], batch, spatial, heads, ch, levels,
-                                Q, P, G, outputs[0], stream);
-      return b200_msda_f16(inputs[0], shapes, inputs[2], inputs[3], inputs[4], batch, spatial, heads, ch, levels, Q, P,
-                           G, outputs[0], stream);
+      if (use_h2 && g.C % 2 == 0)
+        return b200_msda_f16_h2(inputs[0], shapes, inputs[2], inputs[3], inputs[4], g.B, g.S, g.M, g.C, g.L, g.Q, g.P,
+                                g.G, outputs[0], stream);
+      return b200_msda_f16(inputs[0], shapes, inputs[2], inputs[3], inputs[4], g.B, g.S, g.M, g.C, g.L, g.Q, g.P, g.G,
+                           outputs[0], stream);
     case 2: {  // kINT8; reference points stay fp16 or fp32 (…Plugin.cpp:168-176)
       if (in[2].type != 0 && in[2].type != 1) return B200_ERR_UNSUPPORTED;
-      const size_t ws = workspace ? b200_msda_i8_workspace_size(batch, spatial, heads, ch, levels, P, G) : 0;
+      const size_t ws = workspace ? b200_msda_i8_workspace_size(g.B, g.S, g.M, g.C, g.L, g.P, g.G) : 0;
       if (ws) {
         const int st = b200_msda_i8_ws(static_cast<const int8_t *>(inputs[0]), in[0].scale, shapes, inputs[2],
                                        in[2].type == 1, static_cast<const int8_t *>(inputs[3]), in[3].scale,
-                                       static_cast<const int8_t *>(inputs[4]), in[4].scale, batch, spatial, heads, ch,
-                                       levels, Q, P, G, static_cast<int8_t *>(outputs[0]), out[0].scale, workspace, ws,
+                                       static_cast<const int8_t *>(inputs[4]), in[4].scale, g.B, g.S, g.M, g.C, g.L,
+                                       g.Q, g.P, g.G, static_cast<int8_t *>(outputs[0]), out[0].scale, workspace, ws,
                                        nullptr, stream);
         if (st != B200_ERR_UNSUPPORTED) return st;
       }
       return b200_msda_i8(static_cast<const int8_t *>(inputs[0]), in[0].scale, shapes, inputs[2], in[2].type == 1,
                           static_cast<const int8_t *>(inputs[3]), in[3].scale, static_cast<const int8_t *>(inputs[4]),
-                          in[4].scale, batch, spatial, heads, ch, levels, Q, P, G, static_cast<int8_t *>(outputs[0]),
+                          in[4].scale, g.B, g.S, g.M, g.C, g.L, g.Q, g.P, g.G, static_cast<int8_t *>(outputs[0]),
                           out[0].scale, stream);
     }
     default:
@@ -73,18 +78,16 @@ int b200_msda_enqueue(const b200_tensor_desc *in, const b200_tensor_desc *out, c
 // getWorkspaceSize mirror for the MSDA plugin shell: dimensions only, like the TensorRT call.
 size_t b200_msda_enqueue_workspace_size(const b200_tensor_desc *in) {
   if (!in) return 0;
-  const int levels = in[1].dims.d[0];
-  if (levels <= 0) return 0;
+  if (in[1].dims.d[0] <= 0) return 0;
   if (in[0].type != 2) return 0;  // kINT8 only
-  return b200_msda_i8_workspace_size(in[0].dims.d[0], in[0].dims.d[1], in[0].dims.d[2], in[0].dims.d[3], levels,
-                                     in[4].dims.d[3] / levels, in[2].dims.d[3] / 2);
+  const MsdaGeom g = msda_desc_geom(in, in[1].dims.d[0]);
+  return b200_msda_i8_workspace_size(g.B, g.S, g.M, g.C, g.L, g.P, g.G);
 }
 
 int b200_msda_supports_format(int pos, const b200_tensor_desc *io, int nb_inputs, int nb_outputs) {
   if (!io || nb_inputs != 5 || nb_outputs != 1) return 0;
-  const int levels = io[1].dims.d[0] > 0 ? io[1].dims.d[0] : 1;
-  const int channels = io[0].dims.d[3], point_num = io[4].dims.d[3] / levels;
-  const bool int8_ok = (channels % 4 == 0) && (point_num % 4 == 0);
+  const MsdaGeom g = msda_desc_geom(io, io[1].dims.d[0] > 0 ? io[1].dims.d[0] : 1);
+  const bool int8_ok = (g.C % 4 == 0) && (g.P % 4 == 0);
   const bool linear = io[pos].format == 0;
   switch (pos) {
     case 0: return linear && (io[0].type == 0 || io[0].type == 1 || (io[0].type == 2 && int8_ok));

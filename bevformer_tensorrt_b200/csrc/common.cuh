@@ -22,6 +22,9 @@ inline int check_launch() {
   return cudaGetLastError() == cudaSuccess ? B200_OK : B200_ERR_LAUNCH;
 }
 
+// workspace carve-outs start on 256-byte boundaries
+inline size_t align256(size_t b) { return (b + 255) / 256 * 256; }
+
 constexpr unsigned kFullMask = 0xffffffffu;
 
 // ---- 128-bit read-only loads -------------------------------------------------------------------------------

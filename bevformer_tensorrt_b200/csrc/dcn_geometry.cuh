@@ -55,7 +55,6 @@ inline void dcn_set_layer(P &p, const DcnGeom &g) {
   p.dil_w = g.dil_w, p.Ho = g.Ho, p.Wo = g.Wo;
 }
 
-inline size_t align256(size_t b) { return (b + 255) / 256 * 256; }
 inline unsigned grid_for(long long n) { return static_cast<unsigned>(n / 256 + 1 < (1 << 20) ? n / 256 + 1 : (1 << 20)); }
 
 // dcn_fused.cu

@@ -22,11 +22,12 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "msda_geometry.cuh"
 #include "msda_index.cuh"
 
 namespace b200 {
 
-constexpr int kMaxLevels = 16;
+constexpr int kMaxLevels = kMsdaMaxLevels;
 constexpr int kThreads = 256;
 #ifndef B200_MSDA_MIN_BLOCKS
 #define B200_MSDA_MIN_BLOCKS 3
@@ -73,10 +74,6 @@ static int msda_batch_units() {
   }
   return v;
 }
-
-// msda_res.cu
-int msda_res_f16(const void *value, const int32_t *shapes, const void *ref, const void *off, const void *logits, int B, int S,
-                 int M, int C, int L, int Q, int P, int G, void *out, int4 *trace, int cap_bytes, cudaStream_t s);
 
 struct MsdaParams {
   const void *value;
@@ -918,22 +915,16 @@ __global__ void msda_index_kernel(const int32_t *shapes, const T *ref, const T *
 // ---------------------------------------------------------------------------------------------------------------
 // Host side
 // ---------------------------------------------------------------------------------------------------------------
-static int validate(const MsdaParams &p) {
-  if (!p.value || !p.shapes || !p.ref || !p.off || !p.logits || !(p.out || (p.accum && p.mask)))
-    return B200_ERR_BAD_PARAM;
-  if (p.B <= 0 || p.S <= 0 || p.M <= 0 || p.C <= 0 || p.L <= 0 || p.Q <= 0 || p.P <= 0 || p.G <= 0)
-    return B200_ERR_BAD_PARAM;
-  if (p.L > kMaxLevels) return B200_ERR_UNSUPPORTED;
-  if ((static_cast<long long>(p.S) + 1) * p.M * p.C * 4 >= (1ll << 31)) return B200_ERR_BAD_PARAM;
-  return B200_OK;
-}
-
 template <typename T, typename R, int C, int ROUNDS, int MODE, int EPI>
 static int launch_gather(const MsdaParams &p, cudaStream_t s) {
   constexpr int LPI = C / Io<T, 0>::kVec;
   constexpr int IPB = (32 / LPI) * (kThreads / 32);
   const long long blocks = (p.items + IPB - 1) / IPB;
   if (blocks > 0x7fffffffll) return B200_ERR_BAD_PARAM;
+  auto launch = [s](void (*kernel)(const MsdaParams), long long grid, int threads, const MsdaParams &prm) {
+    kernel<<<static_cast<unsigned>(grid), threads, 0, s>>>(prm);
+    return check_launch();
+  };
   // Batched launch (visibility scan over UPW units per warp): the FP32 / FP16 plugin op at <= 2 rounds, which covers
   // every BEVFormer shape (NP = 32 points: 2 rounds FP16, 1 round FP32). The traced instantiation follows the same
   // switch, so the index records the parity tests read come out of whichever kernel the plugin op runs.
@@ -943,37 +934,29 @@ static int launch_gather(const MsdaParams &p, cudaStream_t s) {
       const long long bb = (blocks + upw - 1) / upw;
       MsdaParams q = p;
       q.unit_stride = (cfg >> 8) & 1;
-      if (p.trace != nullptr) {
-        if (upw == 4) msda_gather_kernel<T, R, C, ROUNDS, 0, 0, true, 4><<<static_cast<unsigned>(bb), kThreads, 0, s>>>(q);
-        else msda_gather_kernel<T, R, C, ROUNDS, 0, 0, true, 2><<<static_cast<unsigned>(bb), kThreads, 0, s>>>(q);
-      } else if (msda_gather_variant() == 1) {  // batched scan AND 2 CTAs per SM (128-register budget)
-        if (upw == 4) msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 4, 2><<<static_cast<unsigned>(bb), kThreads, 0, s>>>(q);
-        else msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 2, 2><<<static_cast<unsigned>(bb), kThreads, 0, s>>>(q);
-      } else {
-        if (upw == 4) msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 4><<<static_cast<unsigned>(bb), kThreads, 0, s>>>(q);
-        else msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 2><<<static_cast<unsigned>(bb), kThreads, 0, s>>>(q);
-      }
-      return check_launch();
+      if (p.trace != nullptr)
+        return launch(upw == 4 ? msda_gather_kernel<T, R, C, ROUNDS, 0, 0, true, 4>
+                               : msda_gather_kernel<T, R, C, ROUNDS, 0, 0, true, 2>, bb, kThreads, q);
+      if (msda_gather_variant() == 1)  // batched scan AND 2 CTAs per SM (128-register budget)
+        return launch(upw == 4 ? msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 4, 2>
+                               : msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 2, 2>, bb, kThreads, q);
+      return launch(upw == 4 ? msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 4>
+                             : msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 2>, bb, kThreads, q);
     }
   }
   if constexpr (EPI == 0 && MODE == 0) {
-    if (p.trace != nullptr) {
-      msda_gather_kernel<T, R, C, ROUNDS, MODE, 0, true><<<static_cast<unsigned>(blocks), kThreads, 0, s>>>(p);
-      return check_launch();
-    }
+    if (p.trace != nullptr) return launch(msda_gather_kernel<T, R, C, ROUNDS, MODE, 0, true>, blocks, kThreads, p);
   }
   // Gather-depth variants of the same plugin op (one-unit grid, untraced launches): see the kernel's header comment.
   if constexpr (EPI == 0 && MODE == 0 && ROUNDS <= 2 && !std::is_same<T, int8_t>::value) {
-    const unsigned gb = static_cast<unsigned>(blocks);
     switch (msda_gather_variant()) {
-      case 1: msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 1, 2, 1><<<gb, kThreads, 0, s>>>(p); return check_launch();
-      case 2: msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 1, 2, 4><<<gb, kThreads, 0, s>>>(p); return check_launch();
+      case 1: return launch(msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 1, 2, 1>, blocks, kThreads, p);
+      case 2: return launch(msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 1, 2, 4>, blocks, kThreads, p);
       case 3: {  // 128-thread CTAs, 5 per SM
         constexpr int IPB128 = (32 / LPI) * (128 / 32);
         const long long b128 = (p.items + IPB128 - 1) / IPB128;
         if (b128 > 0x7fffffffll) break;
-        msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 1, 5, 2, 128><<<static_cast<unsigned>(b128), 128, 0, s>>>(p);
-        return check_launch();
+        return launch(msda_gather_kernel<T, R, C, ROUNDS, 0, 0, false, 1, 5, 2, 128>, b128, 128, p);
       }
       default: break;
     }
@@ -981,20 +964,15 @@ static int launch_gather(const MsdaParams &p, cudaStream_t s) {
   // The fused spatial-cross-attention forms follow the same switch with one alternative: any non-zero gather variant runs
   // them at 2 CTAs per SM (same source, 128-register budget: a chunk's 16 tap loads in flight per warp).
   if constexpr (EPI != 0 && MODE == 0 && ROUNDS <= 2) {
-    if (msda_gather_variant() != 0) {
-      msda_gather_kernel<T, R, C, ROUNDS, 0, EPI, false, 1, 2, 1><<<static_cast<unsigned>(blocks), kThreads, 0, s>>>(p);
-      return check_launch();
-    }
+    if (msda_gather_variant() != 0)
+      return launch(msda_gather_kernel<T, R, C, ROUNDS, 0, EPI, false, 1, 2, 1>, blocks, kThreads, p);
   }
-  msda_gather_kernel<T, R, C, ROUNDS, MODE, EPI><<<static_cast<unsigned>(blocks), kThreads, 0, s>>>(p);
-  return check_launch();
+  return launch(msda_gather_kernel<T, R, C, ROUNDS, MODE, EPI>, blocks, kThreads, p);
 }
 
 template <typename T, typename R>
 static int launch_generic(const MsdaParams &p, cudaStream_t s) {
-  const long long n = p.items * p.C;
-  const long long blocks = (n + kThreads - 1) / kThreads;
-  msda_generic_kernel<T, R><<<static_cast<unsigned>(blocks < (1 << 20) ? blocks : (1 << 20)), kThreads, 0, s>>>(p);
+  msda_generic_kernel<T, R><<<msda_grid_for(p.items * p.C), kThreads, 0, s>>>(p);
   return check_launch();
 }
 
@@ -1010,85 +988,95 @@ static int dispatch_rounds(const MsdaParams &p, cudaStream_t s) {
 }
 
 template <typename T, typename R, int MODE, int EPI = 0>
-static int dispatch(const MsdaParams &p, cudaStream_t s) {
-  const int st = validate(p);
-  if (st != B200_OK) return st;
-  const bool aligned = (reinterpret_cast<uintptr_t>(p.value) % 16 == 0) &&
-                       (reinterpret_cast<uintptr_t>(p.off) % 16 == 0) &&
-                       (reinterpret_cast<uintptr_t>(p.logits) % 16 == 0) &&
-                       (reinterpret_cast<uintptr_t>(p.out) % 16 == 0) &&
-                       (reinterpret_cast<uintptr_t>(p.accum) % 16 == 0);
-  const bool g_ok = p.G == 1 || p.G == 2 || p.G == 4;
-  const bool ref_aligned = reinterpret_cast<uintptr_t>(p.ref) % 16 == 0 && reinterpret_cast<uintptr_t>(p.shapes) % 8 == 0;
-  if (aligned && ref_aligned && p.P % 4 == 0 && g_ok && p.L * p.P / 4 <= kMaxChunks) {
-    // every BEVFormer variant has embed_dims / num_heads = 256 / 8 = 32 channels per head
-    if (p.C == 32) return dispatch_rounds<T, R, 32, MODE, EPI>(p, s);
-  }
+static int dispatch(const MsdaParams &p, const MsdaGeom &g, cudaStream_t s) {
+  // every BEVFormer variant has embed_dims / num_heads = 256 / 8 = 32 channels per head
+  if (msda_aligned({p.value, p.off, p.logits, p.out, p.accum, p.ref}, 16) && msda_aligned({p.shapes}, 8) &&
+      msda_lane_group_shape(g, kMaxChunks * 4))
+    return dispatch_rounds<T, R, 32, MODE, EPI>(p, s);
   return EPI == 0 ? launch_generic<T, R>(p, s) : B200_ERR_UNSUPPORTED;
 }
 
 static MsdaParams make_params(const void *value, const int32_t *shapes, const void *ref, const void *off,
-                              const void *logits, int B, int S, int M, int C, int L, int Q, int P, int G, void *out) {
+                              const void *logits, void *out, const MsdaGeom &g) {
   MsdaParams p{};
   p.value = value, p.shapes = shapes, p.ref = ref, p.off = off, p.logits = logits, p.out = out;
-  p.B = B, p.S = S, p.M = M, p.C = C, p.L = L, p.Q = Q, p.P = P, p.G = G;
-  p.items = static_cast<long long>(B) * Q * M;
+  msda_set_dims(p, g);
+  p.items = static_cast<long long>(g.B) * g.Q * g.M;
   p.scale_value = p.scale_offset = p.scale_weight = p.scale_out = 1.f;
   return p;
 }
 
-static MsdaParams make_i8_params(const void *value, float scale_value, const int32_t *shapes, const void *ref,
-                                 int ref_is_half, const void *off, float scale_offset, const void *logits,
-                                 float scale_weight, int B, int S, int M, int C, int L, int Q, int P, int G, void *out,
-                                 float scale_out) {
-  MsdaParams p = make_params(value, shapes, ref, off, logits, B, S, M, C, L, Q, P, G, out);
-  p.scale_value = scale_value, p.scale_offset = scale_offset, p.scale_weight = scale_weight, p.scale_out = scale_out;
-  p.ref_is_half = ref_is_half;
-  return p;
-}
-
-// The plugin op of each dtype family, untraced (records == nullptr) or traced: argument checks, zero-fill of the
-// records, kernel selection and launch happen here only, so a trace entry runs the kernel its plugin op runs.
-static int op_prologue(MsdaParams &p, int32_t *records, cudaStream_t s) {
-  const int st = validate(p);
+// Argument checks of every forward entry, and the zero-fill of a traced launch's records. Each plugin op checks, selects
+// its kernel and launches in one place, untraced (records == nullptr) or traced, so a trace entry runs the kernel its
+// plugin op runs.
+static int op_prologue(MsdaParams &p, const MsdaGeom &g, int32_t *records, cudaStream_t s) {
+  if (!p.value || !p.shapes || !p.ref || !p.off || !p.logits || !(p.out || (p.accum && p.mask)))
+    return B200_ERR_BAD_PARAM;
+  const int st = msda_check_dims(g);
   if (st != B200_OK || !records) return st;
-  if (cudaMemsetAsync(records, 0, static_cast<size_t>(p.items) * p.L * p.P * 16, s) != cudaSuccess) return B200_ERR_LAUNCH;
+  if (cudaMemsetAsync(records, 0, static_cast<size_t>(p.items) * g.L * g.P * 16, s) != cudaSuccess) return B200_ERR_LAUNCH;
   p.trace = reinterpret_cast<int4 *>(records);
   return B200_OK;
 }
 
-static int msda_f32_op(MsdaParams p, int32_t *records, cudaStream_t s) {
-  const int st = op_prologue(p, records, s);
-  return st != B200_OK ? st : dispatch<float, float, 0>(p, s);
+// FP32, and BF16 value / offsets / logits / out with FP32 reference points (a bf16 reference point would move the
+// sampling position by up to 2^-9 of the level's extent; BF16 takes FP16's kernel selection, without the FP16 mode and
+// path switches).
+template <typename T, typename R>
+static int msda_exact_op(MsdaParams p, const MsdaGeom &g, int32_t *records, cudaStream_t s) {
+  const int st = op_prologue(p, g, records, s);
+  return st != B200_OK ? st : dispatch<T, R, 0>(p, g, s);
 }
 
 // Resident-tail kernel only with exact arithmetic; a traced launch is always exact (the gather kernel's DBG
 // instantiation exists for MODE 0 only).
-static int msda_f16_op(MsdaParams p, int32_t *records, cudaStream_t s) {
-  int st = op_prologue(p, records, s);
+static int msda_f16_op(MsdaParams p, const MsdaGeom &g, int32_t *records, cudaStream_t s) {
+  int st = op_prologue(p, g, records, s);
   if (st != B200_OK) return st;
   const bool mixed = g_f16_mode.load(std::memory_order_relaxed) != 0;
   if (g_f16_path.load(std::memory_order_relaxed) && !mixed) {
-    st = msda_res_f16(p.value, p.shapes, p.ref, p.off, p.logits, p.B, p.S, p.M, p.C, p.L, p.Q, p.P, p.G, p.out, p.trace,
+    st = msda_res_f16(p.value, p.shapes, p.ref, p.off, p.logits, p.out, p.trace, g,
                       g_res_cap_bytes.load(std::memory_order_relaxed), s);
     if (st != B200_ERR_UNSUPPORTED) return st;
   }
-  return mixed && !records ? dispatch<__half, __half, 1>(p, s) : dispatch<__half, __half, 0>(p, s);
+  return mixed && !records ? dispatch<__half, __half, 1>(p, g, s) : dispatch<__half, __half, 0>(p, g, s);
 }
 
-// BF16 value / offsets / logits / out with FP32 reference points (a bf16 reference point would move the sampling
-// position by up to 2^-9 of the level's extent). FP16's kernel selection; the FP16 mode and path switches do not apply.
-static int msda_bf16_op(MsdaParams p, int32_t *records, cudaStream_t s) {
-  const int st = op_prologue(p, records, s);
-  return st != B200_OK ? st : dispatch<__nv_bfloat16, float, 0>(p, s);
+// The C-ABI entries of each family: the plugin ops and their trace twins, which require `records`.
+using MsdaOp = int (*)(MsdaParams, const MsdaGeom &, int32_t *, cudaStream_t);
+
+template <MsdaOp OP, bool TRACE = false>
+static int plugin_entry(const void *value, const int32_t *shapes, const void *ref, const void *off, const void *logits,
+                        void *out, int32_t *records, const MsdaGeom &g, void *stream) {
+  if (TRACE && !records) return B200_ERR_BAD_PARAM;
+  return OP(make_params(value, shapes, ref, off, logits, out, g), g, records, static_cast<cudaStream_t>(stream));
 }
 
-static int msda_i8_op(MsdaParams p, int32_t *records, cudaStream_t s) {
-  if (p.C % 4 != 0 || p.P % 4 != 0) return B200_ERR_UNSUPPORTED;  // …Plugin.cpp:151-156
-  if (!(p.scale_out > 0.f)) return B200_ERR_BAD_PARAM;
-  const int st = op_prologue(p, records, s);
+template <bool TRACE = false>
+static int i8_entry(const int8_t *value, float scale_value, const int32_t *shapes, const void *ref, int ref_is_half,
+                    const int8_t *off, float scale_offset, const int8_t *logits, float scale_weight, int8_t *out,
+                    float scale_out, int32_t *records, const MsdaGeom &g, void *stream) {
+  if (TRACE && !records) return B200_ERR_BAD_PARAM;
+  if (g.C % 4 != 0 || g.P % 4 != 0) return B200_ERR_UNSUPPORTED;  // …Plugin.cpp:151-156
+  if (!(scale_out > 0.f)) return B200_ERR_BAD_PARAM;
+  MsdaParams p = make_params(value, shapes, ref, off, logits, out, g);
+  p.scale_value = scale_value, p.scale_offset = scale_offset, p.scale_weight = scale_weight, p.scale_out = scale_out;
+  p.ref_is_half = ref_is_half;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int st = op_prologue(p, g, records, s);
   if (st != B200_OK) return st;
-  return p.ref_is_half ? dispatch<int8_t, __half, 0>(p, s) : dispatch<int8_t, float, 0>(p, s);
+  return ref_is_half ? dispatch<int8_t, __half, 0>(p, g, s) : dispatch<int8_t, float, 0>(p, g, s);
+}
+
+// The fused spatial-cross-attention forms: EPI 1 camera-summed (accum), EPI 2 camera-shared (slots).
+template <typename T, typename R, int EPI>
+static int sca_entry(const void *value, const int32_t *shapes, const void *ref, const void *off, const void *logits,
+                     const float *bev_mask, float *accum, const MsdaGeom &g, void *stream) {
+  MsdaParams p = make_params(value, shapes, ref, off, logits, nullptr, g);
+  p.mask = bev_mask, p.accum = accum;
+  if (EPI == 2) p.items = static_cast<long long>(g.Q) * g.M;  // one item per (query, head); cameras are looped inside
+  const int st = op_prologue(p, g, nullptr, static_cast<cudaStream_t>(stream));
+  return st != B200_OK ? st : dispatch<T, R, 0, EPI>(p, g, static_cast<cudaStream_t>(stream));
 }
 
 }  // namespace b200
@@ -1117,20 +1105,17 @@ int b200_msda_f32(const float *value, const int32_t *spatial_shapes, const float
                   const float *sampling_offsets, const float *attn_weight, int batch, int spatial_size, int num_heads,
                   int channels, int num_levels, int num_query, int num_point, int points_per_group, float *out,
                   void *stream) {
-  return msda_f32_op(make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                                 spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                                 out),
-                     nullptr, static_cast<cudaStream_t>(stream));
+  return plugin_entry<msda_exact_op<float, float>>(value, spatial_shapes, reference_points, sampling_offsets,
+      attn_weight, out, nullptr,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_f16(const void *value, const int32_t *spatial_shapes, const void *reference_points,
                   const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size, int num_heads,
                   int channels, int num_levels, int num_query, int num_point, int points_per_group, void *out,
                   void *stream) {
-  return msda_f16_op(make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                                 spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                                 out),
-                     nullptr, static_cast<cudaStream_t>(stream));
+  return plugin_entry<msda_f16_op>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, out, nullptr,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_f16_h2(const void *value, const int32_t *spatial_shapes, const void *reference_points,
@@ -1146,89 +1131,72 @@ int b200_msda_bf16(const void *value, const int32_t *spatial_shapes, const float
                    const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size, int num_heads,
                    int channels, int num_levels, int num_query, int num_point, int points_per_group, void *out,
                    void *stream) {
-  return msda_bf16_op(make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                                  spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                                  out),
-                      nullptr, static_cast<cudaStream_t>(stream));
+  return plugin_entry<msda_exact_op<__nv_bfloat16, float>>(value, spatial_shapes, reference_points, sampling_offsets,
+      attn_weight, out, nullptr,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_i8(const int8_t *value, float scale_value, const int32_t *spatial_shapes, const void *reference_points,
                  int ref_is_half, const int8_t *sampling_offsets, float scale_offset, const int8_t *attn_weight,
                  float scale_weight, int batch, int spatial_size, int num_heads, int channels, int num_levels,
                  int num_query, int num_point, int points_per_group, int8_t *out, float scale_out, void *stream) {
-  return msda_i8_op(make_i8_params(value, scale_value, spatial_shapes, reference_points, ref_is_half, sampling_offsets,
-                                   scale_offset, attn_weight, scale_weight, batch, spatial_size, num_heads, channels,
-                                   num_levels, num_query, num_point, points_per_group, out, scale_out),
-                    nullptr, static_cast<cudaStream_t>(stream));
+  return i8_entry(value, scale_value, spatial_shapes, reference_points, ref_is_half, sampling_offsets, scale_offset,
+      attn_weight, scale_weight, out, scale_out, nullptr,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_sca_f32(const float *value, const int32_t *spatial_shapes, const float *reference_points,
                       const float *sampling_offsets, const float *attn_weight, const float *bev_mask, int batch,
                       int spatial_size, int num_heads, int channels, int num_levels, int num_query, int num_point,
                       int points_per_group, float *accum, void *stream) {
-  MsdaParams p = make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                             spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                             nullptr);
-  p.mask = bev_mask, p.accum = accum;
-  return dispatch<float, float, 0, 1>(p, static_cast<cudaStream_t>(stream));
+  return sca_entry<float, float, 1>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, bev_mask,
+      accum, msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group),
+      stream);
 }
 
 int b200_msda_sca_f16(const void *value, const int32_t *spatial_shapes, const void *reference_points,
                       const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
                       int spatial_size, int num_heads, int channels, int num_levels, int num_query, int num_point,
                       int points_per_group, float *accum, void *stream) {
-  MsdaParams p = make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                             spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                             nullptr);
-  p.mask = bev_mask, p.accum = accum;
-  return dispatch<__half, __half, 0, 1>(p, static_cast<cudaStream_t>(stream));
+  return sca_entry<__half, __half, 1>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, bev_mask,
+      accum, msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group),
+      stream);
 }
 
 int b200_msda_sca_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
                        const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
                        int spatial_size, int num_heads, int channels, int num_levels, int num_query, int num_point,
                        int points_per_group, float *accum, void *stream) {
-  MsdaParams p = make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                             spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                             nullptr);
-  p.mask = bev_mask, p.accum = accum;
-  return dispatch<__nv_bfloat16, float, 0, 1>(p, static_cast<cudaStream_t>(stream));
+  return sca_entry<__nv_bfloat16, float, 1>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight,
+      bev_mask, accum,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_sca_shared_f32(const float *value, const int32_t *spatial_shapes, const float *reference_points,
                              const float *sampling_offsets, const float *attn_weight, const float *bev_mask,
                              int batch, int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                              int num_point, int points_per_group, float *slots, void *stream) {
-  MsdaParams p = make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                             spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                             nullptr);
-  p.mask = bev_mask, p.accum = slots;
-  p.items = static_cast<long long>(num_query) * num_heads;  // one item per (query, head); cameras are looped inside
-  return dispatch<float, float, 0, 2>(p, static_cast<cudaStream_t>(stream));
+  return sca_entry<float, float, 2>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, bev_mask,
+      slots, msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group),
+      stream);
 }
 
 int b200_msda_sca_shared_f16(const void *value, const int32_t *spatial_shapes, const void *reference_points,
                              const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
                              int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                              int num_point, int points_per_group, float *slots, void *stream) {
-  MsdaParams p = make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                             spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                             nullptr);
-  p.mask = bev_mask, p.accum = slots;
-  p.items = static_cast<long long>(num_query) * num_heads;
-  return dispatch<__half, __half, 0, 2>(p, static_cast<cudaStream_t>(stream));
+  return sca_entry<__half, __half, 2>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, bev_mask,
+      slots, msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group),
+      stream);
 }
 
 int b200_msda_sca_shared_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
                               const void *sampling_offsets, const void *attn_weight, const float *bev_mask, int batch,
                               int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                               int num_point, int points_per_group, float *slots, void *stream) {
-  MsdaParams p = make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                             spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                             nullptr);
-  p.mask = bev_mask, p.accum = slots;
-  p.items = static_cast<long long>(num_query) * num_heads;
-  return dispatch<__nv_bfloat16, float, 0, 2>(p, static_cast<cudaStream_t>(stream));
+  return sca_entry<__nv_bfloat16, float, 2>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight,
+      bev_mask, slots,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 // The plugin ops with the trace switch on: same kernel selection, plus one record per point.
@@ -1236,33 +1204,27 @@ int b200_msda_f32_trace(const float *value, const int32_t *spatial_shapes, const
                         const float *sampling_offsets, const float *attn_weight, int batch, int spatial_size,
                         int num_heads, int channels, int num_levels, int num_query, int num_point,
                         int points_per_group, float *out, int32_t *records, void *stream) {
-  if (!records) return B200_ERR_BAD_PARAM;
-  return msda_f32_op(make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                                 spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                                 out),
-                     records, static_cast<cudaStream_t>(stream));
+  return plugin_entry<msda_exact_op<float, float>, true>(value, spatial_shapes, reference_points, sampling_offsets,
+      attn_weight, out, records,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_f16_trace(const void *value, const int32_t *spatial_shapes, const void *reference_points,
                         const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size,
                         int num_heads, int channels, int num_levels, int num_query, int num_point,
                         int points_per_group, void *out, int32_t *records, void *stream) {
-  if (!records) return B200_ERR_BAD_PARAM;
-  return msda_f16_op(make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                                 spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                                 out),
-                     records, static_cast<cudaStream_t>(stream));
+  return plugin_entry<msda_f16_op, true>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, out,
+      records, msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group),
+      stream);
 }
 
 int b200_msda_bf16_trace(const void *value, const int32_t *spatial_shapes, const float *reference_points,
                          const void *sampling_offsets, const void *attn_weight, int batch, int spatial_size,
                          int num_heads, int channels, int num_levels, int num_query, int num_point,
                          int points_per_group, void *out, int32_t *records, void *stream) {
-  if (!records) return B200_ERR_BAD_PARAM;
-  return msda_bf16_op(make_params(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, batch,
-                                  spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-                                  out),
-                      records, static_cast<cudaStream_t>(stream));
+  return plugin_entry<msda_exact_op<__nv_bfloat16, float>, true>(value, spatial_shapes, reference_points,
+      sampling_offsets, attn_weight, out, records,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_i8_trace(const int8_t *value, float scale_value, const int32_t *spatial_shapes,
@@ -1270,11 +1232,9 @@ int b200_msda_i8_trace(const int8_t *value, float scale_value, const int32_t *sp
                        float scale_offset, const int8_t *attn_weight, float scale_weight, int batch, int spatial_size,
                        int num_heads, int channels, int num_levels, int num_query, int num_point, int points_per_group,
                        int8_t *out, float scale_out, int32_t *records, void *stream) {
-  if (!records) return B200_ERR_BAD_PARAM;
-  return msda_i8_op(make_i8_params(value, scale_value, spatial_shapes, reference_points, ref_is_half, sampling_offsets,
-                                   scale_offset, attn_weight, scale_weight, batch, spatial_size, num_heads, channels,
-                                   num_levels, num_query, num_point, points_per_group, out, scale_out),
-                    records, static_cast<cudaStream_t>(stream));
+  return i8_entry<true>(value, scale_value, spatial_shapes, reference_points, ref_is_half, sampling_offsets,
+      scale_offset, attn_weight, scale_weight, out, scale_out, records,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_debug_indices(int dtype, const int32_t *spatial_shapes, const void *reference_points,
@@ -1283,7 +1243,7 @@ int b200_msda_debug_indices(int dtype, const int32_t *spatial_shapes, const void
   if (!spatial_shapes || !reference_points || !sampling_offsets || !records) return B200_ERR_BAD_PARAM;
   const long long n = static_cast<long long>(batch) * num_query * num_heads * num_levels * num_point;
   if (n <= 0) return B200_ERR_BAD_PARAM;
-  const unsigned blocks = static_cast<unsigned>((n + 255) / 256 < (1 << 20) ? (n + 255) / 256 : (1 << 20));
+  const unsigned blocks = msda_grid_for(n);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (dtype == 0)
     msda_index_kernel<float><<<blocks, 256, 0, s>>>(spatial_shapes, static_cast<const float *>(reference_points),

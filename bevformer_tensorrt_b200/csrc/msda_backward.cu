@@ -43,12 +43,13 @@
 // trees, fixed loops): the same bits on every run and for every subset of requested gradients. grad_value is summed
 // with float atomics and is not (as in mmcv).
 #include "common.cuh"
+#include "msda_geometry.cuh"
 #include "msda_index.cuh"
 
 namespace b200 {
 namespace {
 
-constexpr int kBwMaxLevels = 16;
+constexpr int kBwMaxLevels = kMsdaMaxLevels;
 constexpr int kBwThreads = 256;
 constexpr int kBwC32MaxPoints = 64;  // the C = 32 kernel parks 3 floats per (item, point) in shared memory
 
@@ -463,74 +464,56 @@ __global__ void msda_bw_f32_round_kernel(const float *in, T *out, long long n) {
 }
 
 // ---- host ------------------------------------------------------------------------------------------------------------
-unsigned grid_for(long long n) {
-  const long long b = (n + kBwThreads - 1) / kBwThreads;
-  return static_cast<unsigned>(b < (1 << 20) ? (b > 0 ? b : 1) : (1 << 20));
-}
-size_t align256(size_t b) { return (b + 255) / 256 * 256; }
-
-// The forward's envelope (validate() in msda.cu), without the pointers.
-int bw_check_dims(int B, int S, int M, int C, int L, int Q, int P, int G) {
-  if (B <= 0 || S <= 0 || M <= 0 || C <= 0 || L <= 0 || Q <= 0 || P <= 0 || G <= 0) return B200_ERR_BAD_PARAM;
-  if (L > kBwMaxLevels) return B200_ERR_UNSUPPORTED;
-  if ((static_cast<long long>(S) + 1) * M * C * 4 >= (1ll << 31)) return B200_ERR_BAD_PARAM;
-  return B200_OK;
-}
-
 // Workspace: [fp32 grad_value accumulator, FP16 only][fp32 grad_reference_points partials, one per (item, group, xy)]
 struct BwPlan {
   size_t gv, ref, total;
 };
-BwPlan bw_plan(bool f16, int B, int S, int M, int C, int Q, int G) {
+BwPlan bw_plan(bool f16, const MsdaGeom &g) {
   BwPlan pl{};
   pl.gv = 0;
-  pl.ref = f16 ? align256(static_cast<size_t>(B) * S * M * C * 4) : 0;
-  pl.total = pl.ref + align256(static_cast<size_t>(B) * Q * M * G * 2 * 4);
+  pl.ref = f16 ? align256(static_cast<size_t>(g.B) * g.S * g.M * g.C * 4) : 0;
+  pl.total = pl.ref + align256(static_cast<size_t>(g.B) * g.Q * g.M * g.G * 2 * 4);
   return pl;
 }
 
-// The kernel selection rule, in one place: the lane-group kernel takes the shapes of every BEVFormer call site (32
-// channels per head, points in chunks of 4, 1 / 2 / 4 reference points per query, at most 64 points per item) when every
-// tensor it moves as 128-bit words is 16-byte aligned; everything else runs the one-thread-per-item kernel.
-bool msda_bw_takes_c32(const MsdaBwParams &p) {
-  const void *ptrs[] = {p.value, p.ref, p.off, p.logits, p.gout, p.gv_acc, p.goff, p.glog};
-  for (const void *q : ptrs)
-    if (reinterpret_cast<uintptr_t>(q) % 16) return false;
-  return p.C == 32 && p.P % 4 == 0 && (p.G == 1 || p.G == 2 || p.G == 4) && p.L * p.P <= kBwC32MaxPoints;
+// The kernel selection rule, in one place: the lane-group kernel takes the lane-group shape with at most 64 points per
+// item when every tensor it moves as 128-bit words is 16-byte aligned; everything else runs the one-thread-per-item
+// kernel.
+bool msda_bw_takes_c32(const MsdaBwParams &p, const MsdaGeom &g) {
+  return msda_aligned({p.value, p.ref, p.off, p.logits, p.gout, p.gv_acc, p.goff, p.glog}, 16) &&
+         msda_lane_group_shape(g, kBwC32MaxPoints);
 }
 
 // EPI 0: the plugin op (mask null, gout = grad_out in T). EPI 1 / 2: the fused SCA forms (gout = grad_slots, fp32
 // [Q, M*C]; mask = bev_mask [B, Q]), lane-group kernel only: shapes outside its envelope return B200_ERR_UNSUPPORTED.
+// T: storage type of value, offsets, logits and their gradients; R: of the reference points and their gradient.
 template <typename T, int EPI, typename R = typename BwRef<T>::type>
-int msda_backward(const T *value, const int32_t *shapes, const R *ref, const T *off, const T *logits, const float *mask,
-                  const void *gout, T *gvalue, R *gref, T *goff, T *glog, void *workspace, int B, int S, int M, int C,
-                  int L, int Q, int P, int G, cudaStream_t s) {
+int msda_backward(const void *value, const int32_t *shapes, const void *ref, const void *off, const void *logits,
+                  const float *mask, const void *gout, void *gvalue, void *gref, void *goff, void *glog,
+                  void *workspace, const MsdaGeom &g, void *stream) {
   constexpr bool kF16 = sizeof(T) == 2;  // FP16 or BF16: grad_value is accumulated in the fp32 workspace
   if (!value || !shapes || !ref || !off || !logits || !gout || !workspace) return B200_ERR_BAD_PARAM;
   if (EPI != 0 && !mask) return B200_ERR_BAD_PARAM;
-  int st = bw_check_dims(B, S, M, C, L, Q, P, G);
+  int st = msda_check_dims(g);
   if (st != B200_OK) return st;
-  const void *ptrs[] = {value, off, logits, gvalue, goff, glog};
-  for (const void *q : ptrs)
-    if (reinterpret_cast<uintptr_t>(q) % sizeof(T)) return B200_ERR_BAD_PARAM;
-  if (reinterpret_cast<uintptr_t>(ref) % sizeof(R) || reinterpret_cast<uintptr_t>(gref) % sizeof(R)) return B200_ERR_BAD_PARAM;
-  if (reinterpret_cast<uintptr_t>(gout) % (EPI == 0 ? sizeof(T) : sizeof(float)) ||
-      reinterpret_cast<uintptr_t>(mask) % 4)
+  if (!msda_aligned({value, off, logits, gvalue, goff, glog}, sizeof(T)) || !msda_aligned({ref, gref}, sizeof(R)) ||
+      !msda_aligned({gout}, EPI == 0 ? sizeof(T) : sizeof(float)) || !msda_aligned({mask, shapes}, 4) ||
+      !msda_aligned({workspace}, 256))
     return B200_ERR_BAD_PARAM;
-  if (reinterpret_cast<uintptr_t>(shapes) % 4 || reinterpret_cast<uintptr_t>(workspace) % 256) return B200_ERR_BAD_PARAM;
   if (!gvalue && !gref && !goff && !glog) return B200_OK;
 
-  const BwPlan pl = bw_plan(kF16, B, S, M, C, Q, G);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const BwPlan pl = bw_plan(kF16, g);
   char *ws = static_cast<char *>(workspace);
-  const long long nv = static_cast<long long>(B) * S * M * C;
+  const long long nv = static_cast<long long>(g.B) * g.S * g.M * g.C;
   MsdaBwParams p{};
   p.value = value, p.shapes = shapes, p.ref = ref, p.off = off, p.logits = logits, p.gout = gout, p.mask = mask;
-  p.B = B, p.S = S, p.M = M, p.C = C, p.L = L, p.Q = Q, p.P = P, p.G = G;
-  p.items = static_cast<long long>(EPI == 2 ? 1 : B) * Q * M;
-  p.gv_acc = gvalue ? (kF16 ? reinterpret_cast<float *>(ws + pl.gv) : reinterpret_cast<float *>(gvalue)) : nullptr;
+  msda_set_dims(p, g);
+  p.items = static_cast<long long>(EPI == 2 ? 1 : g.B) * g.Q * g.M;
+  p.gv_acc = gvalue ? (kF16 ? reinterpret_cast<float *>(ws + pl.gv) : static_cast<float *>(gvalue)) : nullptr;
   p.goff = goff, p.glog = glog;
   p.ref_part = gref ? reinterpret_cast<float *>(ws + pl.ref) : nullptr;
-  const bool c32 = msda_bw_takes_c32(p);
+  const bool c32 = msda_bw_takes_c32(p, g);
   if (EPI != 0 && !c32) return B200_ERR_UNSUPPORTED;
   if (p.gv_acc && cudaMemsetAsync(p.gv_acc, 0, static_cast<size_t>(nv) * 4, s) != cudaSuccess) return B200_ERR_LAUNCH;
 
@@ -538,24 +521,25 @@ int msda_backward(const T *value, const int32_t *shapes, const R *ref, const T *
     constexpr int IPB = (32 / (32 / BwIo<T>::kVec)) * (kBwThreads / 32);
     const long long blocks = (p.items + IPB - 1) / IPB;
     if (blocks > 0x7fffffffll) return B200_ERR_BAD_PARAM;
-    const size_t smem = static_cast<size_t>(IPB) * L * P * 3 * sizeof(float);
+    const size_t smem = static_cast<size_t>(IPB) * g.L * g.P * 3 * sizeof(float);
     if (cudaFuncSetAttribute(msda_bw_c32_kernel<T, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              IPB * kBwC32MaxPoints * 3 * static_cast<int>(sizeof(float))) != cudaSuccess)
       return B200_ERR_LAUNCH;
     msda_bw_c32_kernel<T, EPI><<<static_cast<unsigned>(blocks), kBwThreads, smem, s>>>(p);
   } else if constexpr (EPI == 0) {
-    msda_bw_generic_kernel<T><<<grid_for(p.items), kBwThreads, 0, s>>>(p);
+    msda_bw_generic_kernel<T><<<msda_grid_for(p.items), kBwThreads, 0, s>>>(p);
   }
   if ((st = check_launch()) != B200_OK) return st;
   if constexpr (kF16) {
     if (gvalue) {
-      msda_bw_f32_round_kernel<T><<<grid_for(nv), kBwThreads, 0, s>>>(p.gv_acc, gvalue, nv);
+      msda_bw_f32_round_kernel<T><<<msda_grid_for(nv), kBwThreads, 0, s>>>(p.gv_acc, static_cast<T *>(gvalue), nv);
       if ((st = check_launch()) != B200_OK) return st;
     }
   }
   if (gref) {
-    const long long nbq = static_cast<long long>(B) * Q;
-    msda_bw_ref_kernel<R><<<grid_for(nbq * 2 * G), kBwThreads, 0, s>>>(p.ref_part, gref, nbq, M, 2 * G);
+    const long long nbq = static_cast<long long>(g.B) * g.Q;
+    msda_bw_ref_kernel<R><<<msda_grid_for(nbq * 2 * g.G), kBwThreads, 0, s>>>(p.ref_part, static_cast<R *>(gref), nbq, g.M,
+                                                                        2 * g.G);
     if ((st = check_launch()) != B200_OK) return st;
   }
   return B200_OK;
@@ -570,11 +554,12 @@ extern "C" {
 
 size_t b200_msda_backward_workspace_size(int dtype, int batch, int spatial_size, int num_heads, int channels,
                                          int num_levels, int num_query, int num_point, int points_per_group) {
-  if ((dtype != 0 && dtype != 1 && dtype != 7) || bw_check_dims(batch, spatial_size, num_heads, channels, num_levels, num_query,
-                                                  num_point, points_per_group) != B200_OK)
-    return 0;
-  return bw_plan(dtype != 0, batch, spatial_size, num_heads, channels, num_query, points_per_group).total;
+  const MsdaGeom g =
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group);
+  if ((dtype != 0 && dtype != 1 && dtype != 7) || msda_check_dims(g) != B200_OK) return 0;
+  return bw_plan(dtype != 0, g).total;
 }
+
 
 int b200_msda_backward_f32(const float *value, const int32_t *spatial_shapes, const float *reference_points,
                            const float *sampling_offsets, const float *attn_weight, const float *grad_output,
@@ -583,9 +568,8 @@ int b200_msda_backward_f32(const float *value, const int32_t *spatial_shapes, co
                            int channels, int num_levels, int num_query, int num_point, int points_per_group,
                            void *stream) {
   return msda_backward<float, 0>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, nullptr,
-                                 grad_output, grad_value, grad_reference_points, grad_sampling_offsets,
-                                 grad_attn_weight, workspace, batch, spatial_size, num_heads, channels, num_levels,
-                                 num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
+      grad_output, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_backward_f16(const void *value, const int32_t *spatial_shapes, const void *reference_points,
@@ -594,13 +578,9 @@ int b200_msda_backward_f16(const void *value, const int32_t *spatial_shapes, con
                            void *grad_attn_weight, void *workspace, int batch, int spatial_size, int num_heads,
                            int channels, int num_levels, int num_query, int num_point, int points_per_group,
                            void *stream) {
-  return msda_backward<__half, 0>(
-      static_cast<const __half *>(value), spatial_shapes, static_cast<const __half *>(reference_points),
-      static_cast<const __half *>(sampling_offsets), static_cast<const __half *>(attn_weight), nullptr, grad_output,
-      static_cast<__half *>(grad_value), static_cast<__half *>(grad_reference_points),
-      static_cast<__half *>(grad_sampling_offsets), static_cast<__half *>(grad_attn_weight), workspace, batch,
-      spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-      static_cast<cudaStream_t>(stream));
+  return msda_backward<__half, 0>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, nullptr,
+      grad_output, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_sca_backward_f32(const float *value, const int32_t *spatial_shapes, const float *reference_points,
@@ -610,9 +590,8 @@ int b200_msda_sca_backward_f32(const float *value, const int32_t *spatial_shapes
                                int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                                int num_point, int points_per_group, void *stream) {
   return msda_backward<float, 1>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, bev_mask,
-                                 grad_slots, grad_value, grad_reference_points, grad_sampling_offsets,
-                                 grad_attn_weight, workspace, batch, spatial_size, num_heads, channels, num_levels,
-                                 num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
+      grad_slots, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_sca_backward_f16(const void *value, const int32_t *spatial_shapes, const void *reference_points,
@@ -621,13 +600,9 @@ int b200_msda_sca_backward_f16(const void *value, const int32_t *spatial_shapes,
                                void *grad_sampling_offsets, void *grad_attn_weight, void *workspace, int batch,
                                int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                                int num_point, int points_per_group, void *stream) {
-  return msda_backward<__half, 1>(
-      static_cast<const __half *>(value), spatial_shapes, static_cast<const __half *>(reference_points),
-      static_cast<const __half *>(sampling_offsets), static_cast<const __half *>(attn_weight), bev_mask, grad_slots,
-      static_cast<__half *>(grad_value), static_cast<__half *>(grad_reference_points),
-      static_cast<__half *>(grad_sampling_offsets), static_cast<__half *>(grad_attn_weight), workspace, batch,
-      spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-      static_cast<cudaStream_t>(stream));
+  return msda_backward<__half, 1>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, bev_mask,
+      grad_slots, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_sca_shared_backward_f32(const float *value, const int32_t *spatial_shapes, const float *reference_points,
@@ -637,9 +612,8 @@ int b200_msda_sca_shared_backward_f32(const float *value, const int32_t *spatial
                                       int batch, int spatial_size, int num_heads, int channels, int num_levels,
                                       int num_query, int num_point, int points_per_group, void *stream) {
   return msda_backward<float, 2>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, bev_mask,
-                                 grad_slots, grad_value, grad_reference_points, grad_sampling_offsets,
-                                 grad_attn_weight, workspace, batch, spatial_size, num_heads, channels, num_levels,
-                                 num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
+      grad_slots, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_sca_shared_backward_f16(const void *value, const int32_t *spatial_shapes, const void *reference_points,
@@ -648,13 +622,9 @@ int b200_msda_sca_shared_backward_f16(const void *value, const int32_t *spatial_
                                       void *grad_sampling_offsets, void *grad_attn_weight, void *workspace, int batch,
                                       int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                                       int num_point, int points_per_group, void *stream) {
-  return msda_backward<__half, 2>(
-      static_cast<const __half *>(value), spatial_shapes, static_cast<const __half *>(reference_points),
-      static_cast<const __half *>(sampling_offsets), static_cast<const __half *>(attn_weight), bev_mask, grad_slots,
-      static_cast<__half *>(grad_value), static_cast<__half *>(grad_reference_points),
-      static_cast<__half *>(grad_sampling_offsets), static_cast<__half *>(grad_attn_weight), workspace, batch,
-      spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group,
-      static_cast<cudaStream_t>(stream));
+  return msda_backward<__half, 2>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight, bev_mask,
+      grad_slots, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 // BF16: value, offsets, logits, grad_output and their gradients in bf16; reference points and their gradient in fp32.
@@ -664,12 +634,9 @@ int b200_msda_backward_bf16(const void *value, const int32_t *spatial_shapes, co
                             void *grad_attn_weight, void *workspace, int batch, int spatial_size, int num_heads,
                             int channels, int num_levels, int num_query, int num_point, int points_per_group,
                             void *stream) {
-  using B = __nv_bfloat16;
-  return msda_backward<B, 0>(
-      static_cast<const B *>(value), spatial_shapes, reference_points, static_cast<const B *>(sampling_offsets),
-      static_cast<const B *>(attn_weight), nullptr, grad_output, static_cast<B *>(grad_value), grad_reference_points,
-      static_cast<B *>(grad_sampling_offsets), static_cast<B *>(grad_attn_weight), workspace, batch, spatial_size,
-      num_heads, channels, num_levels, num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
+  return msda_backward<__nv_bfloat16, 0>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight,
+      nullptr, grad_output, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_sca_backward_bf16(const void *value, const int32_t *spatial_shapes, const float *reference_points,
@@ -678,12 +645,9 @@ int b200_msda_sca_backward_bf16(const void *value, const int32_t *spatial_shapes
                                 void *grad_sampling_offsets, void *grad_attn_weight, void *workspace, int batch,
                                 int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                                 int num_point, int points_per_group, void *stream) {
-  using B = __nv_bfloat16;
-  return msda_backward<B, 1>(
-      static_cast<const B *>(value), spatial_shapes, reference_points, static_cast<const B *>(sampling_offsets),
-      static_cast<const B *>(attn_weight), bev_mask, grad_slots, static_cast<B *>(grad_value), grad_reference_points,
-      static_cast<B *>(grad_sampling_offsets), static_cast<B *>(grad_attn_weight), workspace, batch, spatial_size,
-      num_heads, channels, num_levels, num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
+  return msda_backward<__nv_bfloat16, 1>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight,
+      bev_mask, grad_slots, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 int b200_msda_sca_shared_backward_bf16(const void *value, const int32_t *spatial_shapes,
@@ -693,12 +657,9 @@ int b200_msda_sca_shared_backward_bf16(const void *value, const int32_t *spatial
                                        void *grad_attn_weight, void *workspace, int batch, int spatial_size,
                                        int num_heads, int channels, int num_levels, int num_query, int num_point,
                                        int points_per_group, void *stream) {
-  using B = __nv_bfloat16;
-  return msda_backward<B, 2>(
-      static_cast<const B *>(value), spatial_shapes, reference_points, static_cast<const B *>(sampling_offsets),
-      static_cast<const B *>(attn_weight), bev_mask, grad_slots, static_cast<B *>(grad_value), grad_reference_points,
-      static_cast<B *>(grad_sampling_offsets), static_cast<B *>(grad_attn_weight), workspace, batch, spatial_size,
-      num_heads, channels, num_levels, num_query, num_point, points_per_group, static_cast<cudaStream_t>(stream));
+  return msda_backward<__nv_bfloat16, 2>(value, spatial_shapes, reference_points, sampling_offsets, attn_weight,
+      bev_mask, grad_slots, grad_value, grad_reference_points, grad_sampling_offsets, grad_attn_weight, workspace,
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group), stream);
 }
 
 }  // extern "C"

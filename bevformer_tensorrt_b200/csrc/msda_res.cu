@@ -25,10 +25,11 @@
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint)
 
 #include "common.cuh"
+#include "msda_geometry.cuh"
 
 namespace b200 {
 
-constexpr int kResMaxLevels = 16;
+constexpr int kResMaxLevels = kMsdaMaxLevels;
 constexpr int kBoxRows = 128;  // pixels per TMA box
 #ifndef B200_RES_WARPS
 #define B200_RES_WARPS 24
@@ -308,26 +309,18 @@ static ResEncodeTiledFn res_encoder() {
   return fn;
 }
 
-bool msda_res_supported(int C, int L, int P, int G, int S, int M) {
-  const int NP = L * P;
-  return C == 32 && L >= 1 && L <= kResMaxLevels && P % 4 == 0 && NP <= 32 && (G == 1 || G == 2 || G == 4) &&
-         (static_cast<long long>(S) + 1) * M * 64 < (1ll << 32);
-}
-
-// cap_bytes: shared memory for the tail. Returns B200_ERR_UNSUPPORTED when the shape is outside the envelope.
-int msda_res_f16(const void *value, const int32_t *shapes, const void *ref, const void *off, const void *logits, int B, int S,
-                 int M, int C, int L, int Q, int P, int G, void *out, int4 *trace, int cap_bytes, cudaStream_t s) {
-  if (!msda_res_supported(C, L, P, G, S, M)) return B200_ERR_UNSUPPORTED;
-  const uintptr_t al = reinterpret_cast<uintptr_t>(value) | reinterpret_cast<uintptr_t>(off) | reinterpret_cast<uintptr_t>(logits) |
-                       reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(ref);
-  if (al % 16 || reinterpret_cast<uintptr_t>(shapes) % 8) return B200_ERR_UNSUPPORTED;
-  if (static_cast<long long>(B) * S >= (1ll << 31)) return B200_ERR_UNSUPPORTED;
+int msda_res_f16(const void *value, const int32_t *shapes, const void *ref, const void *off, const void *logits,
+                 void *out, int4 *trace, const MsdaGeom &g, int cap_bytes, cudaStream_t s) {
+  // msda_check_dims has bounded L by kResMaxLevels and (S + 1) * M * 64 by 2^30
+  if (!msda_lane_group_shape(g, 32)) return B200_ERR_UNSUPPORTED;
+  if (!msda_aligned({value, off, logits, out, ref}, 16) || !msda_aligned({shapes}, 8)) return B200_ERR_UNSUPPORTED;
+  if (static_cast<long long>(g.B) * g.S >= (1ll << 31)) return B200_ERR_UNSUPPORTED;
   ResEncodeTiledFn encode = res_encoder();
   if (!encode) return B200_ERR_LAUNCH;
   // value viewed as [B*S rows][M*32 halves]; box = the 32 channels of one head x 128 rows, dense in shared memory
   CUtensorMap tm;
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(M) * 32, static_cast<cuuint64_t>(B) * S};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(M) * 64};
+  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(g.M) * 32, static_cast<cuuint64_t>(g.B) * g.S};
+  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(g.M) * 64};
   const cuuint32_t box[2] = {32, kBoxRows};
   const cuuint32_t estr[2] = {1, 1};
   if (encode(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(value), gdim, gstride, box, estr,
@@ -335,34 +328,24 @@ int msda_res_f16(const void *value, const int32_t *shapes, const void *ref, cons
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return B200_ERR_LAUNCH;
 
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   ResParams p{};
   p.value = static_cast<const char *>(value), p.shapes = shapes, p.ref = ref, p.off = off, p.logits = logits, p.out = out;
-  p.B = B, p.S = S, p.M = M, p.Q = Q, p.P = P, p.G = G, p.L = L, p.trace = trace;
-  const int pairs = B * M;
-  p.cpp = pairs >= sms ? 1 : sms / pairs;
-  const int blocks_q = (Q + kResItemsPerBlock - 1) / kResItemsPerBlock;
-  if (p.cpp > blocks_q) p.cpp = blocks_q;
-  const int grid = pairs >= sms ? sms : pairs * p.cpp;
+  p.B = g.B, p.S = g.S, p.M = g.M, p.Q = g.Q, p.P = g.P, p.G = g.G, p.L = g.L, p.trace = trace;
+  const MsdaSlabGrid sg = msda_slab_grid(g, msda_sm_count(), kResItemsPerBlock);
+  p.cpp = sg.cpp;
   // never more rows than the slice has (small shapes), always whole boxes
   int cap_rows = cap_bytes / 64 / kBoxRows * kBoxRows;
-  const int need = (S + kBoxRows - 1) / kBoxRows * kBoxRows;
+  const int need = (g.S + kBoxRows - 1) / kBoxRows * kBoxRows;
   if (cap_rows > need) cap_rows = need;
   if (cap_rows < kBoxRows) cap_rows = kBoxRows;
   p.cap_rows = cap_rows;
   const int smem = cap_rows * 64;
-  if (trace) {
-    if (cudaFuncSetAttribute(msda_res_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-      return B200_ERR_LAUNCH;
-    msda_res_kernel<true><<<grid, kResThreads, smem, s>>>(p, tm);
-  } else {
-    if (cudaFuncSetAttribute(msda_res_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-      return B200_ERR_LAUNCH;
-    msda_res_kernel<false><<<grid, kResThreads, smem, s>>>(p, tm);
-  }
-  return check_launch();
+  auto launch = [&](auto kernel) -> int {
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return B200_ERR_LAUNCH;
+    kernel<<<sg.grid, kResThreads, smem, s>>>(p, tm);
+    return check_launch();
+  };
+  return trace ? launch(msda_res_kernel<true>) : launch(msda_res_kernel<false>);
 }
 
 }  // namespace b200

@@ -30,6 +30,7 @@
 // and a tensor-core variant (mma.sync with the interleaved entry as A fragment, built and measured on B200: 3.3 ms
 // against 1.03 ms) loses to fragment-order loads that touch 4 lines per quarter warp.
 #include "common.cuh"
+#include "msda_geometry.cuh"
 
 namespace b200 {
 
@@ -450,14 +451,14 @@ __global__ void __launch_bounds__(kI8Threads, 1) msda_i8p_kernel(const I8PParams
 // ---------------------------------------------------------------------------------------------------------------
 static std::atomic<int> g_i8_tail_bytes{128 * 1024};  // shared memory of the gather kernel's resident tail
 
-static bool i8p_shape_ok(int C, int L, int P, int G) {
-  const int NP = L * P;
-  return C == 32 && L >= 1 && L <= kV2MaxLevels && P % 4 == 0 && NP >= 16 && NP <= 32 && (G == 1 || G == 2 || G == 4);
+// The packed kernel's shape: at most kV2MaxLevels levels and 16 to 32 points per item.
+static bool i8p_shape_ok(const MsdaGeom &g) {
+  return g.L >= 1 && g.L <= kV2MaxLevels && g.L * g.P >= 16 && msda_lane_group_shape(g, 32);
 }
 
 // Upper bound of the packed stack from the tensor DIMENSIONS only (what getWorkspaceSize sees): both parity copies of
 // every level, sum_l 2 * (H_l/2 + 1) * W_l <= S + 2 * sum_l W_l <= 3 * S entries per (camera, head).
-static size_t i8p_workspace_bound(int B, int S, int M) { return static_cast<size_t>(3) * S * kEB * B * M; }
+static size_t i8p_workspace_bound(const MsdaGeom &g) { return static_cast<size_t>(3) * g.S * kEB * g.B * g.M; }
 
 }  // namespace b200
 
@@ -467,9 +468,11 @@ extern "C" {
 
 size_t b200_msda_i8_workspace_size(int batch, int spatial_size, int num_heads, int channels, int num_levels, int num_point,
                                    int points_per_group) {
-  if (batch <= 0 || num_heads <= 0 || spatial_size <= 0) return 0;
-  if (!i8p_shape_ok(channels, num_levels, num_point, points_per_group)) return 0;
-  return i8p_workspace_bound(batch, spatial_size, num_heads);
+  // no query count: the packed stack does not depend on it
+  const MsdaGeom g = msda_geom(batch, spatial_size, num_heads, channels, num_levels, 0, num_point, points_per_group);
+  if (g.B <= 0 || g.M <= 0 || g.S <= 0) return 0;
+  if (!i8p_shape_ok(g)) return 0;
+  return i8p_workspace_bound(g);
 }
 
 int b200_msda_i8_ws(const int8_t *value, float scale_value, const int32_t *spatial_shapes, const void *reference_points,
@@ -477,37 +480,36 @@ int b200_msda_i8_ws(const int8_t *value, float scale_value, const int32_t *spati
                     float scale_weight, int batch, int spatial_size, int num_heads, int channels, int num_levels,
                     int num_query, int num_point, int points_per_group, int8_t *out, float scale_out, void *workspace,
                     size_t workspace_bytes, int32_t *trace_records, void *stream) {
+  const MsdaGeom g =
+      msda_geom(batch, spatial_size, num_heads, channels, num_levels, num_query, num_point, points_per_group);
   if (!(scale_out > 0.f)) return B200_ERR_BAD_PARAM;
   if (!value || !spatial_shapes || !reference_points || !sampling_offsets || !attn_weight || !out || !workspace)
     return B200_ERR_BAD_PARAM;
-  if (batch <= 0 || spatial_size <= 0 || num_heads <= 0 || num_query <= 0) return B200_ERR_BAD_PARAM;
-  if (!i8p_shape_ok(channels, num_levels, num_point, points_per_group)) return B200_ERR_UNSUPPORTED;
-  if (workspace_bytes < i8p_workspace_bound(batch, spatial_size, num_heads)) return B200_ERR_BAD_PARAM;
-  if (static_cast<long long>(3) * spatial_size * kEB >= (1ll << 31)) return B200_ERR_UNSUPPORTED;  // 32-bit slab offsets
-  const long long items = static_cast<long long>(batch) * num_query * num_heads;
+  if (g.B <= 0 || g.S <= 0 || g.M <= 0 || g.Q <= 0) return B200_ERR_BAD_PARAM;
+  if (!i8p_shape_ok(g)) return B200_ERR_UNSUPPORTED;
+  if (workspace_bytes < i8p_workspace_bound(g)) return B200_ERR_BAD_PARAM;
+  if (static_cast<long long>(3) * g.S * kEB >= (1ll << 31)) return B200_ERR_UNSUPPORTED;  // 32-bit slab offsets
+  const long long items = static_cast<long long>(g.B) * g.Q * g.M;
   const long long blocks = (items + kI8ItemsPerBlock - 1) / kI8ItemsPerBlock;
   if (blocks > 0x7fffffffll) return B200_ERR_UNSUPPORTED;
-  const uintptr_t al = reinterpret_cast<uintptr_t>(value) | reinterpret_cast<uintptr_t>(workspace) |
-                       reinterpret_cast<uintptr_t>(sampling_offsets) | reinterpret_cast<uintptr_t>(attn_weight) |
-                       reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(reference_points);
-  if (al % 16 || reinterpret_cast<uintptr_t>(spatial_shapes) % 4) return B200_ERR_UNSUPPORTED;
+  if (!msda_aligned({value, workspace, sampling_offsets, attn_weight, out, reference_points}, 16) ||
+      !msda_aligned({spatial_shapes}, 4))
+    return B200_ERR_UNSUPPORTED;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 
   // 1. pack: persistent CTAs, 2 rows x 64 pixels x (M*32) bytes of shared memory each
   PackParams pp{};
   pp.value = reinterpret_cast<const char *>(value), pp.packed = static_cast<char *>(workspace), pp.shapes = spatial_shapes;
-  pp.B = batch, pp.S = spatial_size, pp.M = num_heads, pp.L = num_levels;
-  const int smem = 2 * kPackCols * num_heads * 32;
+  pp.B = g.B, pp.S = g.S, pp.M = g.M, pp.L = g.L;
+  const int smem = 2 * kPackCols * g.M * 32;
   if (smem > 200 * 1024) return B200_ERR_UNSUPPORTED;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = msda_sm_count();
   int per_sm = (200 * 1024) / (smem + 2048);
   per_sm = per_sm < 1 ? 1 : (per_sm > 6 ? 6 : per_sm);
-  const unsigned gx = static_cast<unsigned>((sms * per_sm + batch - 1) / batch);
+  const unsigned gx = static_cast<unsigned>((sms * per_sm + g.B - 1) / g.B);
   if (cudaFuncSetAttribute(msda_pack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
     return B200_ERR_LAUNCH;
-  msda_pack_kernel<<<dim3(gx < 1 ? 1 : gx, static_cast<unsigned>(batch)), 256, smem, s>>>(pp);
+  msda_pack_kernel<<<dim3(gx < 1 ? 1 : gx, static_cast<unsigned>(g.B)), 256, smem, s>>>(pp);
   int st = check_launch();
   if (st != B200_OK) return st;
 
@@ -515,22 +517,18 @@ int b200_msda_i8_ws(const int8_t *value, float scale_value, const int32_t *spati
   I8PParams gp{};
   gp.packed = static_cast<const char *>(workspace), gp.ref = reference_points, gp.off = sampling_offsets;
   gp.logits = attn_weight, gp.out = out, gp.shapes = spatial_shapes;
-  gp.B = batch, gp.M = num_heads, gp.Q = num_query, gp.P = num_point, gp.G = points_per_group;
-  gp.NP = num_levels * num_point, gp.L = num_levels;
+  gp.B = g.B, gp.M = g.M, gp.Q = g.Q, gp.P = g.P, gp.G = g.G, gp.NP = g.L * g.P, gp.L = g.L;
   gp.scale_value = scale_value, gp.scale_offset = scale_offset, gp.scale_weight = scale_weight, gp.scale_out = scale_out;
-  const int pairs = batch * num_heads;
-  gp.cpp = pairs >= sms ? 1 : sms / pairs;
-  const int blocks_q = (num_query + kI8ItemsPerBlock - 1) / kI8ItemsPerBlock;
-  if (gp.cpp > blocks_q) gp.cpp = blocks_q;
-  const int grid = pairs >= sms ? sms : pairs * gp.cpp;
+  const MsdaSlabGrid sg = msda_slab_grid(g, sms, kI8ItemsPerBlock);
+  gp.cpp = sg.cpp;
   long long cap = g_i8_tail_bytes.load(std::memory_order_relaxed);
-  const long long need = static_cast<long long>(3) * spatial_size * kEB;  // never more than a whole slab
+  const long long need = static_cast<long long>(3) * g.S * kEB;  // never more than a whole slab
   if (cap > need) cap = (need + 127) / 128 * 128;
   gp.cap_entries = static_cast<int>(cap / kEB);
   const int gsmem = gp.cap_entries * kEB + kI8Warps * kI8ItemsPerWarp * 33 * 16;  // tail + per-warp sample records
   auto launch = [&](auto kern) -> int {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, gsmem) != cudaSuccess) return B200_ERR_LAUNCH;
-    kern<<<grid, kI8Threads, gsmem, s>>>(gp);
+    kern<<<sg.grid, kI8Threads, gsmem, s>>>(gp);
     return check_launch();
   };
   if (trace_records) {
