@@ -70,6 +70,11 @@ __device__ __forceinline__ bool interval_of(const BevPoolArgs &a, int k, int &s,
   return true;
 }
 
+// The thread's lane group in the whole grid, in 64 bits: items * G passes 2^32 long before items passes INT_MAX.
+__device__ __forceinline__ long long group_index(int G) {
+  return (static_cast<long long>(blockIdx.x) * kBevThreads + threadIdx.x) / G;
+}
+
 __device__ __forceinline__ unsigned group_mask(int G) {
   return G == 32 ? kFullMask : ((1u << G) - 1) << ((threadIdx.x & 31) & ~(G - 1));
 }
@@ -81,9 +86,9 @@ __global__ void __launch_bounds__(kBevThreads) bev_pool_kernel(const BevPoolArgs
   using Acc = AccT<T>;
   using P = Pack<T, VEC>;
   const int gl = threadIdx.x & (G - 1);
-  const int k = (blockIdx.x * kBevThreads + threadIdx.x) / G;
+  const long long k = group_index(G);
   int s, e, cell;
-  if (k >= a.I || !interval_of(a, k, s, e, cell)) return;  // uniform within the group
+  if (k >= a.I || !interval_of(a, static_cast<int>(k), s, e, cell)) return;  // uniform within the group
   const unsigned mask = group_mask(G);
   const int c0 = (blockIdx.y * G + gl) * VEC;
   const bool active = c0 < a.C;
@@ -142,9 +147,9 @@ __global__ void __launch_bounds__(kBevThreads) bev_pool_depth_grad_kernel(const 
                                                                           int *__restrict__ point_cell, int G) {
   using P = Pack<T, VEC>;
   const int gl = threadIdx.x & (G - 1);
-  const int k = (blockIdx.x * kBevThreads + threadIdx.x) / G;
+  const long long k = group_index(G);
   int s, e, cell;
-  if (k >= a.I || !interval_of(a, k, s, e, cell)) return;
+  if (k >= a.I || !interval_of(a, static_cast<int>(k), s, e, cell)) return;
   const unsigned mask = group_mask(G);
   const T *og = out_grad + static_cast<size_t>(cell) * a.C;
   for (int base = s; base < e; base += G) {
@@ -184,8 +189,9 @@ __global__ void __launch_bounds__(kBevThreads) bev_pool_feat_grad_kernel(const B
                                                                          T *__restrict__ feat_grad, int G) {
   using P = Pack<T, VEC>;
   const int gl = threadIdx.x & (G - 1);
-  const int j = (blockIdx.x * kBevThreads + threadIdx.x) / G;
-  if (j >= a.P) return;
+  const long long jl = group_index(G);
+  if (jl >= a.P) return;
+  const int j = static_cast<int>(jl);
   const int head = __ldg(order + j);
   if (head < 0 || head >= a.P) return;
   const int rf = __ldg(a.ranks_feat + head);
@@ -239,13 +245,20 @@ dim3 grid_of(long long items, int C, int vec, int G, bool tiled) {
   return dim3(static_cast<unsigned>((items + per_block - 1) / per_block), tiles);
 }
 
+bool aligned(const void *p, size_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
+
+// elem: the byte size of a depth / feat / out element. Every pointer must be aligned to its element.
 int check_args(const void *depth, const void *feat, const void *out, const int32_t *rd, const int32_t *rf,
                const int32_t *rb, const int32_t *st, const int32_t *ln, int C, int P, int I, long long depth_size,
-               long long feat_rows, int out_h, int out_w) {
+               long long feat_rows, int out_h, int out_w, size_t elem) {
   if (C <= 0 || P < 0 || I < 0 || depth_size < 0 || feat_rows < 0 || out_h <= 0 || out_w <= 0) return B200_ERR_BAD_PARAM;
   if (!out || (P > 0 && (!rd || !rf || !rb)) || (I > 0 && (!st || !ln))) return B200_ERR_BAD_PARAM;
   if ((depth_size > 0 && !depth) || (feat_rows > 0 && !feat)) return B200_ERR_BAD_PARAM;
   if (feat_rows > (1ll << 62) / C) return B200_ERR_BAD_PARAM;
+  for (const void *p : {depth, feat, out})
+    if (!aligned(p, elem)) return B200_ERR_BAD_PARAM;
+  for (const int32_t *p : {rd, rf, rb, st, ln})
+    if (!aligned(p, sizeof(int32_t))) return B200_ERR_BAD_PARAM;
   return B200_OK;
 }
 
@@ -271,26 +284,31 @@ int bev_pool_forward(const BevPoolArgs &a, const T *depth, const T *feat, T *out
 }
 
 template <typename T, int VEC>
-int launch_bwd(const BevPoolArgs &a, const int32_t *order, const T *out_grad, const T *depth, const T *feat,
-               T *depth_grad, T *feat_grad, int *point_cell, cudaStream_t s) {
+void launch_depth_grad(const BevPoolArgs &a, const T *out_grad, const T *feat, T *depth_grad, int *point_cell,
+                       cudaStream_t s) {
   const int G = group_size(a.C, VEC);
-  if (a.I > 0) {
-    bev_pool_depth_grad_kernel<T, VEC><<<grid_of(a.I, a.C, VEC, G, false), kBevThreads, 0, s>>>(a, out_grad, feat,
-                                                                                                depth_grad, point_cell, G);
-    const int st = check_launch();
-    if (st != B200_OK) return st;
-  }
-  if (!feat_grad || a.P == 0) return B200_OK;
-  bev_pool_feat_grad_kernel<T, VEC><<<grid_of(a.P, a.C, VEC, G, true), kBevThreads, 0, s>>>(a, order, out_grad, depth,
-                                                                                           point_cell, feat_grad, G);
-  return check_launch();
+  bev_pool_depth_grad_kernel<T, VEC><<<grid_of(a.I, a.C, VEC, G, false), kBevThreads, 0, s>>>(a, out_grad, feat,
+                                                                                              depth_grad, point_cell, G);
 }
 
+template <typename T, int VEC>
+void launch_feat_grad(const BevPoolArgs &a, const int32_t *order, const T *out_grad, const T *depth,
+                      const int *point_cell, T *feat_grad, cudaStream_t s) {
+  const int G = group_size(a.C, VEC);
+  bev_pool_feat_grad_kernel<T, VEC><<<grid_of(a.P, a.C, VEC, G, true), kBevThreads, 0, s>>>(a, order, out_grad, depth,
+                                                                                           point_cell, feat_grad, G);
+}
+
+// Each kernel takes its vector width from the tensors it reads and writes alone, so the depth gradient's lane partition,
+// and with it its bits, does not depend on whether or where a feature gradient is asked for.
 template <typename T>
 int bev_pool_backward(const BevPoolArgs &a, const int32_t *order, const T *out_grad, const T *depth, const T *feat,
                       T *depth_grad, T *feat_grad, void *workspace, size_t workspace_size, void *stream) {
   if (!out_grad || (!depth_grad && !feat_grad)) return B200_ERR_BAD_PARAM;
   if (feat_grad && a.P > 0 && !order) return B200_ERR_BAD_PARAM;
+  if (!aligned(depth_grad, sizeof(T)) || !aligned(feat_grad, sizeof(T)) || !aligned(order, sizeof(int32_t)) ||
+      !aligned(workspace, sizeof(int)))
+    return B200_ERR_BAD_PARAM;
   const size_t ws = b200_bev_pool_backward_workspace_size(a.P);
   if (ws && (!workspace || workspace_size < ws)) return B200_ERR_BAD_PARAM;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -300,13 +318,24 @@ int bev_pool_backward(const BevPoolArgs &a, const int32_t *order, const T *out_g
   if (feat_grad && cudaMemsetAsync(feat_grad, 0, static_cast<size_t>(a.feat_rows) * a.C * sizeof(T), s) != cudaSuccess)
     return B200_ERR_LAUNCH;
   if (ws && cudaMemsetAsync(point_cell, 0xff, ws, s) != cudaSuccess) return B200_ERR_LAUNCH;
-  switch (pick_vec<T>(a.C, {out_grad, feat, feat_grad})) {
-    case 8: if constexpr (sizeof(T) <= 2) return launch_bwd<T, 8>(a, order, out_grad, depth, feat, depth_grad, feat_grad, point_cell, s); break;
-    case 4: return launch_bwd<T, 4>(a, order, out_grad, depth, feat, depth_grad, feat_grad, point_cell, s);
-    case 2: return launch_bwd<T, 2>(a, order, out_grad, depth, feat, depth_grad, feat_grad, point_cell, s);
-    default: break;
+  if (a.I > 0) {
+    switch (pick_vec<T>(a.C, {out_grad, feat})) {
+      case 8: if constexpr (sizeof(T) <= 2) launch_depth_grad<T, 8>(a, out_grad, feat, depth_grad, point_cell, s); break;
+      case 4: launch_depth_grad<T, 4>(a, out_grad, feat, depth_grad, point_cell, s); break;
+      case 2: launch_depth_grad<T, 2>(a, out_grad, feat, depth_grad, point_cell, s); break;
+      default: launch_depth_grad<T, 1>(a, out_grad, feat, depth_grad, point_cell, s); break;
+    }
+    const int st = check_launch();
+    if (st != B200_OK) return st;
   }
-  return launch_bwd<T, 1>(a, order, out_grad, depth, feat, depth_grad, feat_grad, point_cell, s);
+  if (!feat_grad || a.P == 0) return B200_OK;
+  switch (pick_vec<T>(a.C, {out_grad, feat_grad})) {
+    case 8: if constexpr (sizeof(T) <= 2) launch_feat_grad<T, 8>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
+    case 4: launch_feat_grad<T, 4>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
+    case 2: launch_feat_grad<T, 2>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
+    default: launch_feat_grad<T, 1>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
+  }
+  return check_launch();
 }
 
 }  // namespace
@@ -326,7 +355,8 @@ int b200_bev_pool_f32(const float *depth, const float *feat, const int32_t *rank
                       int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
                       int out_height, int out_width, float *out, void *stream) {
   const int st = check_args(depth, feat, out, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths,
-                            channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width);
+                            channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width,
+                            sizeof(float));
   if (st != B200_OK) return st;
   B200_BEV_POOL_ARGS;
   return bev_pool_forward<float>(a, depth, feat, out, 0.f, stream);
@@ -337,7 +367,8 @@ int b200_bev_pool_f16(const void *depth, const void *feat, const int32_t *ranks_
                       int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
                       int out_height, int out_width, void *out, void *stream) {
   const int st = check_args(depth, feat, out, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths,
-                            channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width);
+                            channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width,
+                            sizeof(__half));
   if (st != B200_OK) return st;
   B200_BEV_POOL_ARGS;
   return bev_pool_forward<__half>(a, static_cast<const __half *>(depth), static_cast<const __half *>(feat),
@@ -350,7 +381,8 @@ int b200_bev_pool_i8(const int8_t *depth, float scale_depth, const int8_t *feat,
                      int num_intervals, int64_t depth_size, int64_t feat_rows, int out_height, int out_width,
                      int8_t *out, float scale_out, void *stream) {
   const int st = check_args(depth, feat, out, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths,
-                            channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width);
+                            channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width,
+                            sizeof(int8_t));
   if (st != B200_OK) return st;
   if (channels % 4 != 0) return B200_ERR_UNSUPPORTED;
   B200_BEV_POOL_ARGS;
@@ -370,7 +402,7 @@ int b200_bev_pool_backward_f32(const float *out_grad, const float *depth, const 
                                void *stream) {
   const int st = check_args(depth, feat, out_grad, ranks_depth, ranks_feat, ranks_bev, interval_starts,
                             interval_lengths, channels, num_points, num_intervals, depth_size, feat_rows, out_height,
-                            out_width);
+                            out_width, sizeof(float));
   if (st != B200_OK) return st;
   B200_BEV_POOL_ARGS;
   return bev_pool_backward<float>(a, feat_order, out_grad, depth, feat, depth_grad, feat_grad, workspace,
@@ -385,7 +417,7 @@ int b200_bev_pool_backward_f16(const void *out_grad, const void *depth, const vo
                                void *stream) {
   const int st = check_args(depth, feat, out_grad, ranks_depth, ranks_feat, ranks_bev, interval_starts,
                             interval_lengths, channels, num_points, num_intervals, depth_size, feat_rows, out_height,
-                            out_width);
+                            out_width, sizeof(__half));
   if (st != B200_OK) return st;
   B200_BEV_POOL_ARGS;
   return bev_pool_backward<__half>(a, feat_order, static_cast<const __half *>(out_grad),

@@ -690,7 +690,8 @@ int b200_dcn_enqueue(const b200_tensor_desc *input_desc, const b200_tensor_desc 
  * Numerics: FP32 = the reference kernel's FFMA chain in point order, bit for bit. FP16 accumulates in FP32 and rounds
  * once. INT8 (channels % 4 == 0, else B200_ERR_UNSUPPORTED): exact int32 sum, one multiply by
  * scale_depth * scale_feat / scale_out (evaluated in float on the host), saturate, round half away from zero.
- * Pointers of zero-length arrays may be NULL; any other NULL pointer or a negative size is B200_ERR_BAD_PARAM. */
+ * Pointers of zero-length arrays may be NULL; any other NULL pointer, a pointer not aligned to its element (4 bytes
+ * for float and int32, 2 for half) or a negative size is B200_ERR_BAD_PARAM. */
 int b200_bev_pool_f32(const float *depth, const float *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
                       const int32_t *ranks_bev, const int32_t *interval_starts, const int32_t *interval_lengths,
                       int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,

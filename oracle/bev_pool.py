@@ -1,7 +1,7 @@
 """oracle/bev_pool.py — TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
 ctypes driver for oracle/bev_pool_cpu.c (BEVPoolV2 restated in C: float64 forward / backward, the FP32 forward as an
-fmaf chain, the INT8 forward) and ``RefBevPool``, which calls the reference's own BEVPoolV2 kernels
+fmaf chain, the INT8 forward, the FP32 backward in the kernels' lane partition) and ``RefBevPool``, which calls the reference's own BEVPoolV2 kernels
 (oracle/ref_bev_pool_shim.cu, built into oracle/_ref/libref_bev_pool.so by oracle/bev_pool.mk) on torch CUDA tensors.
 """
 import ctypes
@@ -92,6 +92,23 @@ def bev_pool_backward_f64(out_grad, depth, feat, ranks, out_hw):
     args, keep = _common(ranks, depth.size, rows, C, out_hw)
     dg, fg = np.empty_like(depth), np.empty_like(feat)
     lib().bev_pool_backward_f64(_ptr(og), _ptr(depth), _ptr(feat), *args, _ptr(dg), _ptr(fg))
+    return dg, fg
+
+
+def bev_pool_backward_f32_lanes(out_grad, depth, feat, ranks, out_hw, G, vec, depth_grad=True, feat_grad=True):
+    """The float32 depth / feature gradients as the device kernels compute them for a lane group of ``G`` lanes of
+    ``vec`` channels each (see bev_pool_cpu.c). Returns (depth_grad shaped like depth or None, feat_grad shaped like feat
+    or None), float32. For FP16, pass the widened halves and round the result once with ``np.float16``."""
+    og = np.ascontiguousarray(out_grad, np.float32)
+    depth, feat = np.ascontiguousarray(depth, np.float32), np.ascontiguousarray(feat, np.float32)
+    C, rows = _shape(feat)
+    assert G in (1, 2, 4, 8, 16, 32) and C % vec == 0, (G, vec, C)
+    args, keep = _common(ranks, depth.size, rows, C, out_hw)
+    dg = np.empty_like(depth) if depth_grad else None
+    fg = np.empty_like(feat) if feat_grad else None
+    scratch = np.empty(keep[0].size, np.int64)
+    lib().bev_pool_backward_f32_lanes(_ptr(og), _ptr(depth), _ptr(feat), *args, ctypes.c_int(G), ctypes.c_int(vec),
+                                      None if dg is None else _ptr(dg), None if fg is None else _ptr(fg), _ptr(scratch))
     return dg, fg
 
 

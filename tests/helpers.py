@@ -200,3 +200,11 @@ def make_dcn_inputs(case, seed=0, dtype=torch.float32):
 def fp16_tol(want):
     """FP16-output error budget: 0.5 * spacing_fp16(max|want|) + 1e-3 (see tests/test_dcn_gpu.py)."""
     return 0.5 * float(np.spacing(np.float16(np.abs(want).max()))) + 1e-3
+
+
+def rounding_bound(want, scale, n, dtype):
+    """Per-element bound on a float32-accumulated chain of ``n`` products stored in ``dtype``: half a ulp of ``dtype``
+    at the float64 result ``want``, plus (n + 1) * 2^-24 * ``scale``, where ``scale`` is the same op in float64 on the
+    inputs' magnitudes (it bounds every partial sum of the chain)."""
+    ulp = np.spacing(np.abs(np.asarray(want)).astype(dtype)).astype(np.float64)
+    return 0.5 * ulp + (np.asarray(n, np.float64) + 1.0) * 2.0**-24 * np.asarray(scale, np.float64)

@@ -1,6 +1,7 @@
 """BEVPoolV2 without a GPU: the C oracle against the reference kernels' stored outputs, the Python binding's symbolics,
 registry entries and input checks, the C ABI's argument validation, and the TensorRT shells (tests/mock_trt)."""
 import ctypes
+import ctypes.util
 import os
 import shutil
 import subprocess
@@ -13,7 +14,7 @@ import bevformer_tensorrt_b200 as bt
 from bevformer_tensorrt_b200 import _lib
 from bevformer_tensorrt_b200.workloads import make_bev_pool_inputs, quantize_per_tensor
 from oracle import bev_pool as obev
-from tests.helpers import GOLDEN, golden_index, input_digest
+from tests.helpers import GOLDEN, golden_index, input_digest, rounding_bound
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WORKLOADS = ("tiny", "bevdet_r50", "ref_test")
@@ -52,6 +53,67 @@ def test_oracle_backward_matches_reference_kernel_on_tiny():
     np.testing.assert_allclose(dg.reshape(-1), z["tiny_dgrad"], rtol=1e-5, atol=1e-6)
     np.testing.assert_allclose(fg.reshape(-1), z["tiny_fgrad"], rtol=1e-5, atol=1e-6)
 
+
+
+def _lane_case(C, seed):
+    depth, feat, ranks, hw = make_bev_pool_inputs("tiny", seed)
+    g = torch.Generator().manual_seed(seed + 50)
+    feat = torch.randn(*feat.shape[:-1], C, generator=g)
+    gout = torch.randn(1, hw[0], hw[1], C, generator=g)
+    return gout.numpy(), depth.numpy(), feat.numpy(), [r.numpy() for r in ranks], hw
+
+
+@pytest.mark.parametrize("C,G,vec", [(1, 1, 1), (3, 4, 1), (16, 4, 4), (33, 32, 1), (64, 8, 8), (130, 32, 2),
+                                     (132, 32, 4), (256, 32, 8), (17, 2, 1)])  # fmt: skip
+def test_lane_oracle_within_per_element_bound_of_float64(C, G, vec):
+    """The kernels' lane partition restated in float32 is the backward op: within half a float32 ulp plus (n + 1)
+    roundings of the magnitude sum of float64, element by element (n = C for the depth gradient, the row's point count
+    for the feature gradient). G = 2 at C = 17 is a partition no launch uses: each lane chains many chunks."""
+    og, depth, feat, ranks, hw = _lane_case(C, C)
+    dg, fg = obev.bev_pool_backward_f32_lanes(og, depth, feat, ranks, hw, G, vec)
+    wd, wf = obev.bev_pool_backward_f64(og, depth, feat, ranks, hw)
+    sd, sf = obev.bev_pool_backward_f64(np.abs(og), np.abs(depth), np.abs(feat), ranks, hw)
+    runs = np.bincount(ranks[1], minlength=feat.size // C)
+    assert np.all(np.abs(dg - wd) <= rounding_bound(wd, sd, C, np.float32))
+    assert np.all(np.abs(fg - wf) <= rounding_bound(wf, sf, runs.reshape(feat.shape[:-1] + (1,)), np.float32))
+    assert np.count_nonzero(dg) > 0.9 * ranks[0].size and np.count_nonzero(fg) > 0
+
+
+def _libm_fmaf():
+    f = ctypes.CDLL(ctypes.util.find_library("m")).fmaf
+    f.restype, f.argtypes = ctypes.c_float, [ctypes.c_float] * 3
+    return f
+
+
+def test_lane_oracle_at_one_lane_is_a_plain_fmaf_chain():
+    """G = VEC = 1: the depth gradient is one fmaf chain over c (no butterfly), and the feature gradient one fmaf chain
+    over a row's points in point order, here restated with the C library's fmaf element by element. With one lane the
+    vector width does not reorder anything, so VEC = 2 and 4 give the same bits."""
+    fmaf = _libm_fmaf()
+    C = 12
+    og, depth, feat, ranks, hw = _lane_case(C, 3)
+    rd, rf, rb, st, ln = ranks
+    dg, fg = obev.bev_pool_backward_f32_lanes(og, depth, feat, ranks, hw, 1, 1)
+    ogf, ff, df = og.reshape(-1, C), feat.reshape(-1, C), depth.reshape(-1)
+    want_d, want_f = np.zeros_like(df), np.zeros_like(ff)
+    for k in range(st.size):
+        cell = rb[st[k]]
+        for i in range(st[k], st[k] + ln[k]):
+            acc = 0.0
+            for c in range(C):
+                acc = fmaf(ogf[cell, c], ff[rf[i], c], acc)
+            want_d[rd[i]] = acc
+    for i in np.argsort(rf, kind="stable"):  # the points of each row in point order
+        cell = rb[i]
+        for c in range(C):
+            want_f[rf[i], c] = fmaf(ogf[cell, c], df[rd[i]], want_f[rf[i], c])
+    assert np.array_equal(dg.reshape(-1).view(np.uint32), want_d.view(np.uint32))
+    assert np.array_equal(fg.reshape(-1, C).view(np.uint32), want_f.view(np.uint32))
+    for vec in (2, 4):
+        dv, fv = obev.bev_pool_backward_f32_lanes(og, depth, feat, ranks, hw, 1, vec)
+        assert np.array_equal(dv.view(np.uint32), dg.view(np.uint32)) and np.array_equal(fv.view(np.uint32), fg.view(np.uint32))
+    dv, _ = obev.bev_pool_backward_f32_lanes(og, depth, feat, ranks, hw, 4, 1)
+    assert not np.array_equal(dv.view(np.uint32), dg.view(np.uint32))  # four lanes sum in another order
 
 class _Graph:
     def __init__(self):
@@ -129,6 +191,32 @@ def test_abi_validates_arguments_before_any_cuda_call():
     nb[8] = None  # feat_order, needed for feat_grad
     assert lib.b200_bev_pool_backward_f16(*nb, *ok_dims, p[0], p[1], p[0], 40, None) == 2
 
+
+
+def test_abi_rejects_element_misaligned_pointers_before_any_cuda_call():
+    """A float, half or int32 pointer that is not aligned to its element is B200_ERR_BAD_PARAM, one pointer at a time,
+    in every entry (int8 data needs no alignment; an int8 call fails only on its int32 arrays)."""
+    lib = _lib.load()
+    dims = [16, 10, 3, 100, 50, 8, 8]  # C, P, I, depth_size, feat_rows, out h, out w
+
+    def fake(miss, nbytes):
+        return [ctypes.c_void_p(0x1000 * (i + 1) + (nbytes if i == miss else 0)) for i in range(12)]
+
+    for i in range(7):  # depth, feat, 5 int32 arrays
+        for elem, name in ((2, "b200_bev_pool_f32"), (1, "b200_bev_pool_f16")):
+            p = fake(i, elem if i < 2 else 2)
+            assert getattr(lib, name)(*p[:7], *dims, p[7], None) == 2, (name, i)
+        if i >= 2:
+            p = fake(i, 2)
+            assert lib.b200_bev_pool_i8(p[0], 1.0, p[1], 1.0, *p[2:7], *dims, p[7], 1.0, None) == 2, i
+    for elem, name in ((2, "b200_bev_pool_f32"), (1, "b200_bev_pool_f16")):
+        p = fake(7, elem)  # out
+        assert getattr(lib, name)(*p[:7], *dims, p[7], None) == 2, name
+    for name, elem in (("b200_bev_pool_backward_f32", 2), ("b200_bev_pool_backward_f16", 1)):
+        # out_grad, depth, feat, 5 int32 arrays, feat_order, then depth_grad, feat_grad, workspace
+        for i in range(12):
+            p = fake(i, 2 if 3 <= i <= 8 or i == 11 else elem)
+            assert getattr(lib, name)(*p[:9], *dims, p[9], p[10], p[11], 40, None) == 2, (name, i)
 
 def _desc(dims, type_, fmt=0, scale=1.0):
     d = _lib.TensorDesc()
