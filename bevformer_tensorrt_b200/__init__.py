@@ -97,4 +97,4 @@ __all__ = [
     "set_msda_launch_shape",
     "MSDA_LAUNCH_SHAPES",
 ]
-__version__ = "0.1.1"
+__version__ = "0.1.2"

@@ -94,6 +94,10 @@ SIGNATURES = {
     "b200_grid_sampler_enqueue": (_i, [ctypes.POINTER(TensorDesc), ctypes.POINTER(TensorDesc), ctypes.POINTER(_vp),
                                        ctypes.POINTER(_vp), _vp, _vp, _i, _i, _i]),
     "b200_grid_sampler_supports_format": (_i, [_i, ctypes.POINTER(TensorDesc), _i, _i, _i]),
+    "b200_rotate_enqueue": (_i, [ctypes.POINTER(TensorDesc), ctypes.POINTER(TensorDesc), ctypes.POINTER(_vp),
+                                 ctypes.POINTER(_vp), _vp, _vp, _i, _i]),
+    "b200_rotate_supports_format": (_i, [_i, ctypes.POINTER(TensorDesc), _i, _i, _i]),
+    "b200_dcn_supports_format": (_i, [_i, ctypes.POINTER(TensorDesc), _i, _i, _i, _i]),
     "b200_dcn_enqueue_workspace_size": (ctypes.c_size_t, [ctypes.POINTER(TensorDesc), _ip, _ip, _ip, _i, _i]),
     "b200_dcn_enqueue": (_i, [ctypes.POINTER(TensorDesc), ctypes.POINTER(TensorDesc), ctypes.POINTER(_vp),
                               ctypes.POINTER(_vp), _vp, _vp, _i, _ip, _ip, _ip, _i, _i]),

@@ -1,5 +1,5 @@
 // api.cu — library-level C ABI: identification, status strings, launch counter, and the plugin-shaped
-// enqueue / supportsFormatCombination mirrors for MSDA (reference: multiScaleDeformableAttnPlugin.cpp:71-189).
+// enqueue / supportsFormatCombination mirrors of every plugin (reference: the …Plugin.cpp files named below).
 #include "common.cuh"
 #include "dcn_geometry.cuh"
 #include "msda_geometry.cuh"
@@ -13,13 +13,31 @@ static MsdaGeom msda_desc_geom(const b200_tensor_desc *in, int levels) {
   const int32_t *v = in[0].dims.d;
   return msda_geom(v[0], v[1], v[2], v[3], levels, in[3].dims.d[1], in[4].dims.d[3] / levels, in[2].dims.d[3] / 2);
 }
+
+// The image input of the grid sampler, rotate and DCN plugins: fp32 linear, fp16 linear (kCHW2 for the …TRT2 flavour)
+// or int8 kCHW4 (gridSamplerPlugin.cpp:171-186, rotatePlugin.cpp:122-153, …Conv2dPlugin.cpp:213-250).
+static bool image_format_ok(const b200_tensor_desc &d, int use_h2) {
+  if (d.type == 2) return d.format == 3;
+  if (d.type == 1) return d.format == (use_h2 ? 1 : 0);
+  return d.type == 0 && d.format == 0;
+}
+
+static long long desc_numel(const b200_dims &d) {
+  if (d.nbDims < 0 || d.nbDims > 8) return -1;
+  long long n = 1;
+  for (int i = 0; i < d.nbDims; ++i) {
+    if (d.d[i] < 0) return -1;
+    n *= d.d[i];
+  }
+  return n;
+}
 }  // namespace b200
 
 using namespace b200;
 
 extern "C" {
 
-const char *b200_bev_ops_version(void) { return "b200_bev_ops 0.1.1 sm_90a"; }
+const char *b200_bev_ops_version(void) { return "b200_bev_ops 0.1.2 sm_90a"; }
 
 const char *b200_status_string(int status) {
   switch (status) {
@@ -112,31 +130,20 @@ int b200_grid_sampler_enqueue(const b200_tensor_desc *in, const b200_tensor_desc
   (void)workspace;  // 0 bytes (gridSamplerPlugin.cpp:102-108)
   if (!in || !out || !inputs || !outputs) return B200_ERR_BAD_PARAM;
   const int nb = in[0].dims.nbDims;
-  if (nb != 4 && nb != 5) return B200_ERR_BAD_PARAM;
-  int id[5], gd[5], od[5];
-  for (int i = 0; i < nb; ++i) id[i] = in[0].dims.d[i], gd[i] = in[1].dims.d[i], od[i] = out[0].dims.d[i];
-  switch (in[0].type) {
-    case 0:
-      return b200_grid_sample_f32(static_cast<float *>(outputs[0]), static_cast<const float *>(inputs[0]),
-                                  static_cast<const float *>(inputs[1]), od, id, gd, nb, interpolation_mode, padding_mode,
-                                  align_corners, stream);
-    case 1:
-      if (in[0].format == 1 /* kCHW2 */) {
-        if (nb != 4) return B200_ERR_UNSUPPORTED;
-        return b200_grid_sample_f16_chw2(outputs[0], inputs[0], inputs[1], od, id, gd, nb, interpolation_mode,
-                                         padding_mode, align_corners, stream);
-      }
-      return b200_grid_sample_f16(outputs[0], inputs[0], inputs[1], od, id, gd, nb, interpolation_mode, padding_mode,
-                                  align_corners, stream);
-    case 2:
-      if (nb != 4) return B200_ERR_UNSUPPORTED;
-      return b200_grid_sample_i8_chw4(static_cast<int8_t *>(outputs[0]), out[0].scale,
-                                      static_cast<const int8_t *>(inputs[0]), in[0].scale,
-                                      static_cast<const int8_t *>(inputs[1]), in[1].scale, od, id, gd, nb,
-                                      interpolation_mode, padding_mode, align_corners, stream);
-    default:
-      return B200_ERR_UNSUPPORTED;
-  }
+  if ((nb != 4 && nb != 5) || in[1].dims.nbDims != nb || out[0].dims.nbDims != nb) return B200_ERR_BAD_PARAM;
+  const int *id = in[0].dims.d, *gd = in[1].dims.d, *od = out[0].dims.d;
+  if (in[0].type == 0)
+    return b200_grid_sample_f32(static_cast<float *>(outputs[0]), static_cast<const float *>(inputs[0]),
+                                static_cast<const float *>(inputs[1]), od, id, gd, nb, interpolation_mode, padding_mode,
+                                align_corners, stream);
+  if (in[0].type == 1)
+    return (in[0].format == 1 /* kCHW2 */ ? b200_grid_sample_f16_chw2 : b200_grid_sample_f16)(
+        outputs[0], inputs[0], inputs[1], od, id, gd, nb, interpolation_mode, padding_mode, align_corners, stream);
+  if (in[0].type == 2)
+    return b200_grid_sample_i8_chw4(static_cast<int8_t *>(outputs[0]), out[0].scale, static_cast<const int8_t *>(inputs[0]),
+                                    in[0].scale, static_cast<const int8_t *>(inputs[1]), in[1].scale, od, id, gd, nb,
+                                    interpolation_mode, padding_mode, align_corners, stream);
+  return B200_ERR_UNSUPPORTED;
 }
 
 // io[0] input, io[1] grid, io[2] output. use_h2 = the …TRT2 flavour (FP16 as kCHW2 packets).
@@ -145,9 +152,42 @@ int b200_grid_sampler_supports_format(int pos, const b200_tensor_desc *io, int n
   const b200_tensor_desc &d = io[pos], &x = io[0];
   if (pos != 0) return d.type == x.type && d.format == x.format;
   if (x.dims.nbDims == 5) return (d.type == 0 || d.type == 1) && d.format == 0;  // 5-D: fp32 / fp16 linear (:187-189)
-  if (d.type == 2) return d.format == 3;                                         // int8: kCHW4
-  if (d.type == 1) return d.format == (use_h2 ? 1 : 0);                          // fp16: kCHW2 for …TRT2
-  return d.type == 0 && d.format == 0;
+  return image_format_ok(d, use_h2);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// RotateTRT[2]: enqueue / supportsFormatCombination of the reference (rotatePlugin.cpp:75-113, :122-153). inputs: img
+// [C, H, W], angle [1], center [2]; attribute interpolation. Dispatch: fp32, fp16 linear (kCHW2 for …TRT2), int8 kCHW4
+// with the descriptors' scales and angle / center in the type of the angle descriptor.
+int b200_rotate_enqueue(const b200_tensor_desc *in, const b200_tensor_desc *out, const void *const *inputs,
+                        void *const *outputs, void *workspace, void *stream, int interp, int use_h2) {
+  if (!in || !out || !inputs || !outputs) return B200_ERR_BAD_PARAM;
+  // the kernels read angle[0], center[0..1] and write an image of the input's extent
+  const b200_dims &img = in[0].dims, &o = out[0].dims;
+  if (img.nbDims != 3 || o.nbDims != 3 || o.d[0] != img.d[0] || o.d[1] != img.d[1] || o.d[2] != img.d[2])
+    return B200_ERR_BAD_PARAM;
+  if (desc_numel(in[1].dims) != 1 || desc_numel(in[2].dims) != 2) return B200_ERR_BAD_PARAM;
+  if (in[0].type == 0)
+    return b200_rotate_f32(static_cast<float *>(outputs[0]), static_cast<const float *>(inputs[0]),
+                           static_cast<const float *>(inputs[1]), static_cast<const float *>(inputs[2]), img.d, interp, stream);
+  if (in[0].type == 1)
+    return (use_h2 ? b200_rotate_f16_h2 : b200_rotate_f16)(outputs[0], inputs[0], inputs[1], inputs[2], img.d, interp, stream);
+  if (in[0].type == 2)
+    return b200_rotate_i8(static_cast<int8_t *>(outputs[0]), out[0].scale, static_cast<const int8_t *>(inputs[0]),
+                          in[0].scale, inputs[1], inputs[2], in[1].type == 1, img.d, interp, stream);
+  return B200_ERR_UNSUPPORTED;
+}
+
+// io[0] img, io[1] angle, io[2] center, io[3] output. angle and center are linear in the image's type, or fp32 / fp16
+// of one type for an int8 image.
+int b200_rotate_supports_format(int pos, const b200_tensor_desc *io, int nb_inputs, int nb_outputs, int use_h2) {
+  if (!io || nb_inputs != 3 || nb_outputs != 1 || pos < 0 || pos > 3) return 0;
+  const b200_tensor_desc &d = io[pos], &img = io[0];
+  if (pos == 0) return image_format_ok(d, use_h2);
+  if (pos == 3) return d.type == img.type && d.format == img.format;
+  if (d.format != 0) return 0;
+  if (img.type == 2) return (d.type == 0 || d.type == 1) && d.type == io[1].type;
+  return d.type == img.type;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -168,6 +208,23 @@ size_t b200_dcn_enqueue_workspace_size(const b200_tensor_desc *in, const int32_t
                                             padding[0], dilation[1], dilation[0], groups, deform_groups);
   return b200_dcn_workspace_size(in[0].type == 1, x[0], x[1], x[2], x[3], w[3], w[2], stride[1], stride[0], padding[1],
                                  padding[0], dilation[1], dilation[0]);
+}
+
+// …TRT: fp32 / fp16 linear everywhere. …TRT2 (use_h2): FP16 input, offset and weight as kCHW2 packets, mask / bias /
+// output linear. INT8 (both, when C and Co / groups are multiples of 4): input and weight kCHW4, offset / mask / output
+// int8 linear, bias fp32 or fp16 linear.
+int b200_dcn_supports_format(int pos, const b200_tensor_desc *io, int nb_inputs, int nb_outputs, int groups, int use_h2) {
+  if (!io || (nb_inputs != 4 && nb_inputs != 5) || nb_outputs != 1 || pos < 0 || pos > nb_inputs) return 0;
+  const b200_tensor_desc &d = io[pos], &x = io[0];
+  const bool int8_ok = groups > 0 && x.dims.d[1] % 4 == 0 && (io[nb_inputs].dims.d[1] / groups) % 4 == 0;
+  if (pos == 0) return image_format_ok(d, use_h2) && (d.type != 2 || int8_ok);
+  const bool bias = nb_inputs == 5 && pos == 4;
+  if (x.type == 2) {
+    if (bias) return (d.type == 0 || d.type == 1) && d.format == 0;
+    return d.type == 2 && d.format == (pos == 3 ? 3 : 0);  // weight kCHW4; offset, mask, output linear
+  }
+  if (bias || pos == nb_inputs || pos == 2) return d.type == x.type && d.format == 0;
+  return d.type == x.type && d.format == x.format;  // offset, weight follow the input's format (…Conv2dPlugin.cpp:246-249)
 }
 
 static bool dims_are(const b200_dims &d, long long d0, long long d1, long long d2, long long d3) {
@@ -231,16 +288,6 @@ int b200_dcn_enqueue(const b200_tensor_desc *in, const b200_tensor_desc *out, co
 // BEVPoolV2TRT[2]: enqueue / supportsFormatCombination of the reference (bevPoolPlugin.cpp:71-117, :128-143). The
 // reference takes C from feat.d[3], the interval count from interval_starts.d[0] and the output size from the output
 // descriptor, and checks nothing; here every extent the index checks use comes from the descriptors and must agree.
-static long long desc_numel(const b200_dims &d) {
-  if (d.nbDims < 0 || d.nbDims > 8) return -1;
-  long long n = 1;
-  for (int i = 0; i < d.nbDims; ++i) {
-    if (d.d[i] < 0) return -1;
-    n *= d.d[i];
-  }
-  return n;
-}
-
 int b200_bev_pool_enqueue(const b200_tensor_desc *in, const b200_tensor_desc *out, const void *const *inputs,
                           void *const *outputs, void *workspace, void *stream, int out_height, int out_width) {
   (void)workspace;

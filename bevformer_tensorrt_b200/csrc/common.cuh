@@ -25,6 +25,22 @@ inline int check_launch() {
 // workspace carve-outs start on 256-byte boundaries
 inline size_t align256(size_t b) { return (b + 255) / 256 * 256; }
 
+// Blocks of 256 threads for a grid-stride loop over `threads` items, capped at 2^22.
+inline unsigned capped_blocks(long long threads) {
+  return static_cast<unsigned>(threads / 256 + 1 < (1 << 22) ? threads / 256 + 1 : (1 << 22));
+}
+
+// (pixel, slice) threads: a pixel's channel packets are split into `slices` runs of `cps` packets. Slices double until
+// there are at least min_threads threads and at most max_cps packets per thread, or every packet has its own slice.
+// Returns the blocks of 256 threads.
+inline unsigned plan_slices(long long pixels, int packets, long long min_threads, int max_cps, int &slices, int &cps) {
+  int n = 1;
+  while (n < packets && (pixels * n < min_threads || (packets + n - 1) / n > max_cps)) n <<= 1;
+  cps = (packets + n - 1) / n;
+  slices = (packets + cps - 1) / cps;
+  return capped_blocks(pixels * slices);
+}
+
 constexpr unsigned kFullMask = 0xffffffffu;
 
 // ---- 128-bit read-only loads -------------------------------------------------------------------------------

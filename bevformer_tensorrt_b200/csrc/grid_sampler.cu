@@ -476,53 +476,49 @@ static int launch_gs_tile(const GsParams &p, int mode, cudaStream_t s) {
   return mode == 2 ? launch(grid_sample_2d_tile_kernel<K, true>) : launch(grid_sample_2d_tile_kernel<K, false>);
 }
 
-template <int K>
-static int launch_gs(void *out, const void *in, const void *grid, const int *od, const int *id, const int *gd, int nb,
-                     int interp, int padding, int align, float si, float sg, float so, cudaStream_t s) {
-  if (!out || !in || !grid || !od || !id || !gd) return B200_ERR_BAD_PARAM;
-  if (nb != 4 && nb != 5) return B200_ERR_UNSUPPORTED;  // the reference printf()s and returns (:1959-1961)
+// The one check of a call's dims, which fills p's geometry: N, C and the input extents from input_dims, the output
+// extents from grid_dims (Di = Do = 1 in 2-D), CP = packets of `width` channels. planar3d: the layout has a 3-D kernel.
+// The output dims must be [N, C, grid spatial]: the kernels write that extent whatever output_dims says.
+static int gs_geom(GsParams &p, const int *od, const int *id, const int *gd, int nb, int width, bool planar3d, int interp,
+                   int padding) {
+  // rank 4, or 5 for the linear layouts: the reference printf()s and returns (:1959-1961, :2040-2042)
+  if (nb != 4 && (nb != 5 || !planar3d)) return B200_ERR_UNSUPPORTED;
   if (interp < 0 || interp > 2 || padding < 0 || padding > 2) return B200_ERR_BAD_PARAM;
   for (int i = 0; i < nb; ++i)
     if (id[i] <= 0 || gd[i] <= 0 || od[i] <= 0) return B200_ERR_BAD_PARAM;
   if (gd[0] != id[0] || gd[1] != nb - 2) return B200_ERR_BAD_PARAM;
-  constexpr int W = Pk<K>::W;
-  GsParams p{};
-  p.in = in, p.grid = grid, p.out = out;
-  p.N = id[0], p.C = id[1], p.CP = (id[1] + W - 1) / W;
-  p.interp = interp, p.padding = padding, p.align = align;
-  p.scale_i = si, p.scale_g = sg, p.scale_o = so;
-  if (nb == 4) {
-    p.Di = p.Do = 1, p.Hi = id[2], p.Wi = id[3], p.Ho = gd[2], p.Wo = gd[3];
-  } else {
-    if (K == kF16x2 || K == kI8x4 || interp == 2) return B200_ERR_UNSUPPORTED;  // 3-D: linear layouts, no bicubic
-    p.Di = id[2], p.Hi = id[3], p.Wi = id[4], p.Do = gd[2], p.Ho = gd[3], p.Wo = gd[4];
-  }
+  for (int i = 0; i < nb; ++i)
+    if (od[i] != (i < 2 ? id[i] : gd[i])) return B200_ERR_BAD_PARAM;
+  if (nb == 5 && interp == 2) return B200_ERR_UNSUPPORTED;  // no 3-D bicubic
+  const int s = nb - 4;  // 1 where there is a depth axis
+  p.N = id[0], p.C = id[1], p.CP = (id[1] + width - 1) / width, p.interp = interp, p.padding = padding;
+  p.Di = s ? id[2] : 1, p.Hi = id[2 + s], p.Wi = id[3 + s], p.Do = s ? gd[2] : 1, p.Ho = gd[2 + s], p.Wo = gd[3 + s];
   const long long plane_i = static_cast<long long>(p.Di) * p.Hi * p.Wi;
   const long long plane_o = static_cast<long long>(p.Do) * p.Ho * p.Wo;
-  if (plane_i >= (1ll << 31) || plane_o >= (1ll << 31)) return B200_ERR_BAD_PARAM;
+  return plane_i >= (1ll << 31) || plane_o >= (1ll << 31) ? B200_ERR_BAD_PARAM : B200_OK;
+}
+
+template <int K>
+static int launch_gs(void *out, const void *in, const void *grid, const int *od, const int *id, const int *gd, int nb,
+                     int interp, int padding, int align, float si, float sg, float so, cudaStream_t s) {
+  if (!out || !in || !grid || !od || !id || !gd) return B200_ERR_BAD_PARAM;
+  GsParams p{};
+  const int st = gs_geom(p, od, id, gd, nb, Pk<K>::W, K == kF32 || K == kF16, interp, padding);
+  if (st != B200_OK) return st;
+  p.in = in, p.grid = grid, p.out = out, p.align = align, p.scale_i = si, p.scale_g = sg, p.scale_o = so;
   if (nb == 4 && interp == 0 && g_gs_tile.load(std::memory_order_relaxed)) {
-    const int st = launch_gs_tile<K>(p, g_gs_tile.load(std::memory_order_relaxed), s);
-    if (st != B200_ERR_UNSUPPORTED) return st;
+    const int tst = launch_gs_tile<K>(p, g_gs_tile.load(std::memory_order_relaxed), s);
+    if (tst != B200_ERR_UNSUPPORTED) return tst;
   }
-  // (pixel, slice) threads: about two resident waves of the 132 SMs (4 CTAs x 256 threads each) so that the index
-  // arithmetic of a pixel (~150 instructions) is amortised over as many channel packets as possible, at most 64 per
-  // thread
-  const long long pixels = static_cast<long long>(p.N) * plane_o;
-  int slices = 1;
-  while (slices < p.CP && (pixels * slices < 132ll * 1024 * 2 || (p.CP + slices - 1) / slices > 64)) slices <<= 1;
-  p.cps = (p.CP + slices - 1) / slices;
-  p.slices = (p.CP + p.cps - 1) / p.cps;
-  const long long total = pixels * p.slices;
-  const unsigned blocks = static_cast<unsigned>(total / 256 + 1 < (1 << 22) ? total / 256 + 1 : (1 << 22));
-  if (nb == 4) {
-    if (interp == 0)
-      grid_sample_2d_kernel<K, 0><<<blocks, 256, 0, s>>>(p);
-    else if (interp == 1)
-      grid_sample_2d_kernel<K, 1><<<blocks, 256, 0, s>>>(p);
-    else
-      grid_sample_2d_kernel<K, 2><<<blocks, 256, 0, s>>>(p);
-  } else
-    grid_sample_3d_kernel<(K == kF16 ? kF16 : kF32)><<<blocks, 256, 0, s>>>(p);
+  // about two resident waves of the 132 SMs (4 CTAs x 256 threads each) so that the index arithmetic of a pixel (~150
+  // instructions) is amortised over as many channel packets as possible, at most 64 per thread
+  const unsigned blocks = plan_slices(static_cast<long long>(p.N) * p.Do * p.Ho * p.Wo, p.CP, 132ll * 1024 * 2, 64,
+                                      p.slices, p.cps);
+  const auto kern = nb == 5      ? grid_sample_3d_kernel<(K == kF16 ? kF16 : kF32)>
+                    : interp == 0 ? grid_sample_2d_kernel<K, 0>
+                    : interp == 1 ? grid_sample_2d_kernel<K, 1>
+                                  : grid_sample_2d_kernel<K, 2>;
+  kern<<<blocks, 256, 0, s>>>(p);
   return check_launch();
 }
 
@@ -559,7 +555,6 @@ int b200_grid_sample_i8_chw4(int8_t *output, float scale_o, const int8_t *input,
                              float scale_g, const int *output_dims, const int *input_dims, const int *grid_dims,
                              int nb_dims, int interp, int padding, int align_corners, void *stream) {
   if (!(scale_o > 0.f)) return B200_ERR_BAD_PARAM;
-  if (nb_dims != 4) return B200_ERR_UNSUPPORTED;  // the reference: "input and grid dims should be 4" (:2040-2042)
   return launch_gs<kI8x4>(output, input, grid, output_dims, input_dims, grid_dims, nb_dims, interp, padding,
                           align_corners, scale_i, scale_g, scale_o, static_cast<cudaStream_t>(stream));
 }

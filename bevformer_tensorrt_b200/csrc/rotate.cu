@@ -255,59 +255,52 @@ __global__ void rotate_index_kernel(const RotParams p) {
 }
 
 // ---- host -----------------------------------------------------------------------------------------------------------
-static int rot_check(const void *out, const void *in, const void *angle, const void *center, const int *dims,
-                     int interp) {
-  if (!out || !in || !angle || !center || !dims) return B200_ERR_BAD_PARAM;
-  if (interp < 0 || interp > 1) return B200_ERR_BAD_PARAM;
-  if (dims[0] <= 0 || dims[1] <= 0 || dims[2] <= 0) return B200_ERR_BAD_PARAM;
+// The one check of an image's dims {C, H, W}, which fills p's C, CP (packets of `width` channels), H and W: every extent
+// positive and a plane below 2^31 pixels (the kernels index a plane in int).
+static int rot_geom(RotParams &p, const int *dims, int width) {
+  if (!dims || dims[0] <= 0 || dims[1] <= 0 || dims[2] <= 0) return B200_ERR_BAD_PARAM;
   if (static_cast<long long>(dims[1]) * dims[2] >= (1ll << 31)) return B200_ERR_BAD_PARAM;
+  p.C = dims[0], p.CP = (dims[0] + width - 1) / width, p.H = dims[1], p.W = dims[2];
   return B200_OK;
+}
+
+// The checks both image launchers share; fills the parameters both take.
+static int rot_params(RotParams &p, void *out, const void *in, const void *angle, const void *center, const int *dims,
+                      int width, int interp) {
+  if (!out || !in || !angle || !center || interp < 0 || interp > 1) return B200_ERR_BAD_PARAM;
+  p = RotParams{};
+  p.in = in, p.out = out, p.angle = angle, p.center = center, p.interp = interp;
+  return rot_geom(p, dims, width);
 }
 
 template <int K>
 static int launch_rotate(void *out, const void *in, const void *angle, const void *center, int ac_half,
-                         const int *dims, int interp, float si, float so, float *debug, cudaStream_t s) {
-  const int st = rot_check(out, in, angle, center, dims, interp);
+                         const int *dims, int interp, float si, float so, void *stream) {
+  RotParams p;
+  const int st = rot_params(p, out, in, angle, center, dims, Pk<K>::W, interp);
   if (st != B200_OK) return st;
-  constexpr int PW = Pk<K>::W;
-  RotParams p{};
-  p.in = in, p.out = out, p.angle = angle, p.center = center, p.debug = debug;
-  p.C = dims[0], p.H = dims[1], p.W = dims[2], p.CP = (dims[0] + PW - 1) / PW;
-  p.interp = interp, p.ac_half = ac_half, p.scale_i = si, p.scale_o = so;
-  const long long pixels = static_cast<long long>(p.H) * p.W;
+  p.ac_half = ac_half, p.scale_i = si, p.scale_o = so;
   // enough (pixel, slice) threads to fill 132 SMs a few times over, at most 16 packets per thread
-  int slices = 1;
-  while (slices < p.CP && (pixels * slices < 132ll * 2048 * 4 || (p.CP + slices - 1) / slices > 16)) slices <<= 1;
-  p.cps = (p.CP + slices - 1) / slices;
-  p.slices = (p.CP + p.cps - 1) / p.cps;
-  const long long total = pixels * p.slices;
-  const unsigned blocks = static_cast<unsigned>(total / 256 + 1 < (1 << 22) ? total / 256 + 1 : (1 << 22));
-  if (interp == 0)
-    rotate_planar_kernel<K, 0><<<blocks, 256, 0, s>>>(p);
-  else
-    rotate_planar_kernel<K, 1><<<blocks, 256, 0, s>>>(p);
+  const unsigned blocks = plan_slices(static_cast<long long>(p.H) * p.W, p.CP, 132ll * 2048 * 4, 16, p.slices, p.cps);
+  (interp == 0 ? rotate_planar_kernel<K, 0> : rotate_planar_kernel<K, 1>)<<<blocks, 256, 0,
+                                                                          static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch();
 }
 
 template <int K>
 static int launch_rotate_hwc(void *out, const void *in, const void *angle, const void *center, const int *dims,
-                             int interp, float *debug, cudaStream_t s) {
-  const int st = rot_check(out, in, angle, center, dims, interp);
+                             int interp, void *stream) {
+  RotParams p;
+  const int st = rot_params(p, out, in, angle, center, dims, 1, interp);
   if (st != B200_OK) return st;
-  if (dims[0] % Vec16<K>::N) return B200_ERR_UNSUPPORTED;
+  if (p.C % Vec16<K>::N) return B200_ERR_UNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) return B200_ERR_UNSUPPORTED;
-  RotParams p{};
-  p.in = in, p.out = out, p.angle = angle, p.center = center, p.debug = debug;
-  p.C = dims[0], p.H = dims[1], p.W = dims[2], p.CP = p.C;
-  p.interp = interp, p.ac_half = K == kF16;
+  p.ac_half = K == kF16;
   const int nvec = p.C / Vec16<K>::N;
   p.slices = nvec >= 8 ? 8 : nvec >= 4 ? 4 : nvec >= 2 ? 2 : 1;
-  const long long total = static_cast<long long>(p.H) * p.W * p.slices;
-  const unsigned blocks = static_cast<unsigned>(total / 256 + 1 < (1 << 22) ? total / 256 + 1 : (1 << 22));
-  if (interp == 0)
-    rotate_hwc_kernel<K, 0><<<blocks, 256, 0, s>>>(p);
-  else
-    rotate_hwc_kernel<K, 1><<<blocks, 256, 0, s>>>(p);
+  const unsigned blocks = capped_blocks(static_cast<long long>(p.H) * p.W * p.slices);
+  (interp == 0 ? rotate_hwc_kernel<K, 0> : rotate_hwc_kernel<K, 1>)<<<blocks, 256, 0,
+                                                                    static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch();
 }
 
@@ -319,47 +312,42 @@ extern "C" {
 
 int b200_rotate_f32(float *output, const float *input, const float *angle, const float *center,
                     const int *input_dims, int interp, void *stream) {
-  return launch_rotate<kF32>(output, input, angle, center, 0, input_dims, interp, 1.f, 1.f, nullptr,
-                             static_cast<cudaStream_t>(stream));
+  return launch_rotate<kF32>(output, input, angle, center, 0, input_dims, interp, 1.f, 1.f, stream);
 }
 
 int b200_rotate_f16(void *output, const void *input, const void *angle, const void *center, const int *input_dims,
                     int interp, void *stream) {
-  return launch_rotate<kF16>(output, input, angle, center, 1, input_dims, interp, 1.f, 1.f, nullptr,
-                             static_cast<cudaStream_t>(stream));
+  return launch_rotate<kF16>(output, input, angle, center, 1, input_dims, interp, 1.f, 1.f, stream);
 }
 
 int b200_rotate_f16_h2(void *output, const void *input, const void *angle, const void *center, const int *input_dims,
                        int interp, void *stream) {
-  return launch_rotate<kF16x2>(output, input, angle, center, 1, input_dims, interp, 1.f, 1.f, nullptr,
-                               static_cast<cudaStream_t>(stream));
+  return launch_rotate<kF16x2>(output, input, angle, center, 1, input_dims, interp, 1.f, 1.f, stream);
 }
 
 int b200_rotate_i8(int8_t *output, float scale_o, const int8_t *input, float scale_i, const void *angle,
                    const void *center, int angle_is_half, const int *input_dims, int interp, void *stream) {
   if (!(scale_o > 0.f)) return B200_ERR_BAD_PARAM;
   return launch_rotate<kI8x4>(output, input, angle, center, angle_is_half != 0, input_dims, interp, scale_i, scale_o,
-                              nullptr, static_cast<cudaStream_t>(stream));
+                              stream);
 }
 
 int b200_rotate_hwc(void *output, const void *input, const void *angle, const void *center, int dtype,
                     const int *input_dims, int interp, void *stream) {
-  if (dtype == 0)
-    return launch_rotate_hwc<kF32>(output, input, angle, center, input_dims, interp, nullptr,
-                                   static_cast<cudaStream_t>(stream));
-  if (dtype == 1)
-    return launch_rotate_hwc<kF16>(output, input, angle, center, input_dims, interp, nullptr,
-                                   static_cast<cudaStream_t>(stream));
+  if (dtype == 0) return launch_rotate_hwc<kF32>(output, input, angle, center, input_dims, interp, stream);
+  if (dtype == 1) return launch_rotate_hwc<kF16>(output, input, angle, center, input_dims, interp, stream);
   return B200_ERR_UNSUPPORTED;
 }
 
 int b200_rotate_debug_indices(const float *angle, const float *center, const int *input_dims, float *source_xy,
                               void *stream) {
-  if (!angle || !center || !input_dims || !source_xy) return B200_ERR_BAD_PARAM;
-  if (input_dims[1] <= 0 || input_dims[2] <= 0) return B200_ERR_BAD_PARAM;
+  if (!angle || !center || !source_xy) return B200_ERR_BAD_PARAM;
   RotParams p{};
-  p.angle = angle, p.center = center, p.debug = source_xy, p.H = input_dims[1], p.W = input_dims[2];
+  const int st = rot_geom(p, input_dims, 1);
+  if (st != B200_OK) return st;
   const long long total = static_cast<long long>(p.H) * p.W;
+  if (2 * total >= (1ll << 31)) return B200_ERR_BAD_PARAM;  // the kernel indexes source_xy in int
+  p.angle = angle, p.center = center, p.debug = source_xy;
   rotate_index_kernel<<<static_cast<unsigned>(total / 256 + 1), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch();
 }

@@ -83,44 +83,14 @@ class Plugin final : public IPluginV2DynamicExt {
     return o;
   }
   bool supportsFormatCombination(int32_t pos, const PluginTensorDesc *io, int32_t nbIn, int32_t nbOut) noexcept override {
-    if (op_ == Op::kMSDA)
-      return b200_msda_supports_format(pos, reinterpret_cast<const b200_tensor_desc *>(io), nbIn, nbOut) != 0;
-    if (op_ == Op::kBEVPool)
-      return b200_bev_pool_supports_format(pos, reinterpret_cast<const b200_tensor_desc *>(io), nbIn, nbOut) != 0;
-    if (op_ == Op::kRotate) {  // rotatePlugin.cpp:122-153: img fp32/fp16 linear (kCHW2 for …TRT2) or int8 kCHW4
-      const PluginTensorDesc &d = io[pos], &img = io[0];
-      if (pos == 0) {
-        if (d.type == DataType::kINT8) return d.format == TensorFormat::kCHW4;
-        if (d.type == DataType::kHALF) return d.format == (v2_ ? TensorFormat::kCHW2 : TensorFormat::kLINEAR);
-        return d.type == DataType::kFLOAT && d.format == TensorFormat::kLINEAR;
-      }
-      if (pos == nbIn) return d.type == img.type && d.format == img.format;
-      if (d.format != TensorFormat::kLINEAR) return false;  // angle, center
-      if (img.type == DataType::kINT8)
-        return (d.type == DataType::kFLOAT || d.type == DataType::kHALF) && d.type == io[1].type;
-      return d.type == img.type;
+    const auto *d = reinterpret_cast<const b200_tensor_desc *>(io);
+    switch (op_) {
+      case Op::kMSDA: return b200_msda_supports_format(pos, d, nbIn, nbOut) != 0;
+      case Op::kBEVPool: return b200_bev_pool_supports_format(pos, d, nbIn, nbOut) != 0;
+      case Op::kRotate: return b200_rotate_supports_format(pos, d, nbIn, nbOut, v2_) != 0;
+      case Op::kDCN: return b200_dcn_supports_format(pos, d, nbIn, nbOut, a_.groups, v2_) != 0;
+      default: return b200_grid_sampler_supports_format(pos, d, nbIn, nbOut, v2_) != 0;
     }
-    const PluginTensorDesc &d = io[pos], &x = io[0];
-    if (op_ == Op::kGridSampler2D || op_ == Op::kGridSampler3D)  // gridSamplerPlugin.cpp:168-194
-      return b200_grid_sampler_supports_format(pos, reinterpret_cast<const b200_tensor_desc *>(io), nbIn, nbOut, v2_) != 0;
-    // DCN (…Conv2dPlugin.cpp:213-250). …TRT: fp32 / fp16 linear everywhere. …TRT2 (use_h2): FP16 input, offset and weight
-    // as kCHW2 packets, mask / bias / output linear. INT8 (both): input and weight kCHW4, offset / mask / output int8
-    // linear, bias fp32 or fp16 linear.
-    const bool int8_ok = x.dims.d[1] % 4 == 0 && (io[nbIn].dims.d[1] / a_.groups) % 4 == 0;
-    if (pos == 0) {
-      if (d.type == DataType::kINT8) return d.format == TensorFormat::kCHW4 && int8_ok;
-      if (d.type == DataType::kHALF) return d.format == (v2_ ? TensorFormat::kCHW2 : TensorFormat::kLINEAR);
-      return d.type == DataType::kFLOAT && d.format == TensorFormat::kLINEAR;
-    }
-    if (x.type == DataType::kINT8) {
-      if (nbIn == 5 && pos == 4)
-        return (d.type == DataType::kFLOAT || d.type == DataType::kHALF) && d.format == TensorFormat::kLINEAR;
-      if (pos == 3) return d.type == DataType::kINT8 && d.format == TensorFormat::kCHW4;
-      return d.type == DataType::kINT8 && d.format == TensorFormat::kLINEAR;  // offset, mask, output
-    }
-    (void)nbOut;
-    if ((nbIn == 5 && pos == 4) || pos == nbIn || pos == 2) return d.type == x.type && d.format == TensorFormat::kLINEAR;
-    return d.type == x.type && d.format == x.format;  // offset, weight follow the input's format (…Conv2dPlugin.cpp:246-249)
   }
   void configurePlugin(const DynamicPluginTensorDesc *, int32_t nbIn, const DynamicPluginTensorDesc *, int32_t) noexcept override {
     nb_inputs_ = nbIn;  // DCN: 4 inputs without bias, 5 with (…Conv2dPlugin.cpp:297-299)
@@ -134,35 +104,18 @@ class Plugin final : public IPluginV2DynamicExt {
   }
   int32_t enqueue(const PluginTensorDesc *in, const PluginTensorDesc *out, const void *const *inputs, void *const *outputs,
                   void *workspace, cudaStream_t stream) noexcept override {
-    if (op_ == Op::kMSDA)
-      return b200_msda_enqueue(reinterpret_cast<const b200_tensor_desc *>(in),
-                               reinterpret_cast<const b200_tensor_desc *>(out), inputs, outputs, workspace, stream, v2_);
-    if (op_ == Op::kBEVPool)  // both names run the same kernels
-      return b200_bev_pool_enqueue(reinterpret_cast<const b200_tensor_desc *>(in),
-                                   reinterpret_cast<const b200_tensor_desc *>(out), inputs, outputs, workspace, stream,
-                                   bev_.out_height, bev_.out_width);
-    if (op_ == Op::kRotate) {  // inputs: img, angle, center (rotatePlugin.cpp:75-113)
-      const int *dims = in[0].dims.d;
-      if (in[0].type == DataType::kFLOAT)
-        return b200_rotate_f32(static_cast<float *>(outputs[0]), static_cast<const float *>(inputs[0]),
-                               static_cast<const float *>(inputs[1]), static_cast<const float *>(inputs[2]), dims,
-                               a_.interp, stream);
-      if (in[0].type == DataType::kHALF)
-        return (v2_ ? b200_rotate_f16_h2 : b200_rotate_f16)(outputs[0], inputs[0], inputs[1], inputs[2], dims, a_.interp,
-                                                            stream);
-      if (in[0].type == DataType::kINT8)
-        return b200_rotate_i8(static_cast<int8_t *>(outputs[0]), out[0].scale, static_cast<const int8_t *>(inputs[0]),
-                              in[0].scale, inputs[1], inputs[2], in[1].type == DataType::kHALF, dims, a_.interp, stream);
-      return 1;
+    const auto *i = reinterpret_cast<const b200_tensor_desc *>(in);
+    const auto *o = reinterpret_cast<const b200_tensor_desc *>(out);
+    switch (op_) {
+      case Op::kMSDA: return b200_msda_enqueue(i, o, inputs, outputs, workspace, stream, v2_);
+      case Op::kBEVPool:  // both names run the same kernels
+        return b200_bev_pool_enqueue(i, o, inputs, outputs, workspace, stream, bev_.out_height, bev_.out_width);
+      case Op::kRotate: return b200_rotate_enqueue(i, o, inputs, outputs, workspace, stream, a_.interp, v2_);
+      case Op::kDCN:  // inputs x, offset, mask, weight[, bias]; attributes are ONNX (h, w) pairs, checked against the descriptors
+        return b200_dcn_enqueue(i, o, inputs, outputs, workspace, stream, nb_inputs_, a_.stride, a_.pad, a_.dil, a_.groups,
+                                a_.deform_groups);
+      default: return b200_grid_sampler_enqueue(i, o, inputs, outputs, workspace, stream, a_.interp, a_.padding, a_.align);
     }
-    if (op_ == Op::kGridSampler2D || op_ == Op::kGridSampler3D)
-      return b200_grid_sampler_enqueue(reinterpret_cast<const b200_tensor_desc *>(in),
-                                       reinterpret_cast<const b200_tensor_desc *>(out), inputs, outputs, workspace, stream,
-                                       a_.interp, a_.padding, a_.align);
-    // DCN: inputs x, offset, mask, weight[, bias]; attributes are ONNX (h, w) pairs, checked against the descriptors
-    return b200_dcn_enqueue(reinterpret_cast<const b200_tensor_desc *>(in), reinterpret_cast<const b200_tensor_desc *>(out),
-                            inputs, outputs, workspace, stream, nb_inputs_, a_.stride, a_.pad, a_.dil, a_.groups,
-                            a_.deform_groups);
   }
   // ---- IPluginV2Ext / IPluginV2
   DataType getOutputDataType(int32_t, const DataType *types, int32_t) const noexcept override { return types[0]; }

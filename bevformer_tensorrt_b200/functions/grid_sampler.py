@@ -127,11 +127,22 @@ def unpack_chw(x: torch.Tensor, channels: int) -> torch.Tensor:
     return x.permute(0, 1, 4, 2, 3).reshape(n, cp * width, h, w)[:, :channels].contiguous()
 
 
+def _check_packed(name, input, grid, channels, width, dtype):
+    """Shapes first, then device and dtype: input [N, ceil(channels / width), Hi, Wi, width], grid [N, 1, Ho, Wo, width]
+    of the input's dtype. Returns (n, hi, wi, ho, wo)."""
+    if input.dim() != 5 or input.shape[-1] != width or -(-channels // width) != input.shape[1]:
+        raise ValueError(f"{name}: input must be [N, ceil({channels} / {width}), Hi, Wi, {width}], got {tuple(input.shape)}")
+    if grid.dim() != 5 or grid.shape[0] != input.shape[0] or grid.shape[1] != 1 or grid.shape[-1] != width:
+        raise ValueError(f"{name}: grid must be [{input.shape[0]}, 1, Ho, Wo, {width}], got {tuple(grid.shape)}")
+    if not (input.is_cuda and grid.is_cuda) or input.dtype != dtype or grid.dtype != dtype:
+        raise RuntimeError(f"{name}: input and grid must be {dtype} CUDA tensors")
+    n, _, hi, wi, _ = input.shape
+    return n, hi, wi, grid.shape[2], grid.shape[3]
+
+
 def grid_sampler_chw2(input_chw2, grid_chw2, channels, interpolation_mode: str, padding_mode: str, align_corners: bool):
     """FP16 kCHW2 tensors: input [N, ceil(C/2), Hi, Wi, 2], grid [N, 1, Ho, Wo, 2] = (x, y). Returns kCHW2 output."""
-    assert input_chw2.is_cuda and input_chw2.dtype == torch.float16 and input_chw2.shape[-1] == 2
-    n, _, hi, wi, _ = input_chw2.shape
-    ho, wo = grid_chw2.shape[2:4]
+    n, hi, wi, ho, wo = _check_packed("grid_sampler_chw2", input_chw2, grid_chw2, channels, 2, torch.float16)
     out = torch.empty(n, input_chw2.shape[1], ho, wo, 2, dtype=torch.float16, device=input_chw2.device)
     return _launch("b200_grid_sample_f16_chw2", out, input_chw2.contiguous(), grid_chw2.contiguous(),
                    (n, channels, ho, wo), (n, channels, hi, wi), (n, 2, ho, wo), _MODE[interpolation_mode],
@@ -142,9 +153,7 @@ def grid_sampler_int8(input_chw4, scale_i, grid_chw4, scale_g, scale_o, channels
                       padding_mode: str, align_corners: bool):
     """INT8 kCHW4 tensors with per-tensor scales (real = q*scale): input [N, ceil(C/4), Hi, Wi, 4], grid
     [N, 1, Ho, Wo, 4] = (x, y, 0, 0). Mirrors grid_sample_int8 (gridSamplerKernel.h:20-26). Returns kCHW4 int8."""
-    assert input_chw4.is_cuda and input_chw4.dtype == torch.int8 and input_chw4.shape[-1] == 4
-    n, _, hi, wi, _ = input_chw4.shape
-    ho, wo = grid_chw4.shape[2:4]
+    n, hi, wi, ho, wo = _check_packed("grid_sampler_int8", input_chw4, grid_chw4, channels, 4, torch.int8)
     out = torch.empty(n, input_chw4.shape[1], ho, wo, 4, dtype=torch.int8, device=input_chw4.device)
     return _launch("b200_grid_sample_i8_chw4", out, input_chw4.contiguous(), grid_chw4.contiguous(),
                    (n, channels, ho, wo), (n, channels, hi, wi), (n, 2, ho, wo), _MODE[interpolation_mode],

@@ -39,13 +39,27 @@ def _is_hwc_view(img):
     return c > 1 and img.stride() == (1, w * c, c)
 
 
-def _forward(img, angle, center, interpolation):
+def _check_image(name, img, layout):
+    """A 3-D FP32 / FP16 CUDA image (`layout` names its axes for the message)."""
     if not img.is_cuda:
-        raise RuntimeError("rotate: img must be a CUDA tensor (no CPU fallback exists)")
+        raise RuntimeError(f"{name}: img must be a CUDA tensor (no CPU fallback exists)")
     if img.dim() != 3:
-        raise RuntimeError("rotate: img must be [C, H, W]")
+        raise RuntimeError(f"{name}: img must be {layout}")
     if img.dtype not in (torch.float32, torch.float16):
-        raise _lib.B200OpsError("rotate", 1)
+        raise _lib.B200OpsError(name, 1)
+
+
+def _check_packed(name, img, channels, width, dtype):
+    """Shape first, then device and dtype: img [ceil(channels / width), H, W, width]. Returns the contiguous image."""
+    if img.dim() != 4 or img.shape[-1] != width or -(-channels // width) != img.shape[0]:
+        raise ValueError(f"{name}: img must be [ceil({channels} / {width}), H, W, {width}], got {tuple(img.shape)}")
+    if not img.is_cuda or img.dtype != dtype:
+        raise RuntimeError(f"{name}: img must be a {dtype} CUDA tensor")
+    return img.contiguous()
+
+
+def _forward(img, angle, center, interpolation):
+    _check_image("rotate", img, "[C, H, W]")
     c, h, w = img.shape
     vec = 4 if img.dtype == torch.float32 else 8
     if _is_hwc_view(img) and c % vec == 0 and img.data_ptr() % 16 == 0:
@@ -94,10 +108,7 @@ def rotate2(img, angle, center, interpolation="nearest"):
 
 def rotate_hwc(img_hwc, angle, center, interpolation="nearest"):
     """Channels-last image [H, W, C] (dense), FP32 or FP16; returns [H, W, C]."""
-    if not img_hwc.is_cuda or img_hwc.dim() != 3:
-        raise RuntimeError("rotate_hwc: img must be a CUDA tensor [H, W, C]")
-    if img_hwc.dtype not in (torch.float32, torch.float16):
-        raise _lib.B200OpsError("rotate_hwc", 1)
+    _check_image("rotate_hwc", img_hwc, "[H, W, C]")
     img_hwc = img_hwc.contiguous()
     h, w, c = img_hwc.shape
     angle, center = _scalars(img_hwc, angle, center, img_hwc.dtype)
@@ -110,8 +121,7 @@ def rotate_hwc(img_hwc, angle, center, interpolation="nearest"):
 
 def rotate_chw2(img_chw2, channels, angle, center, interpolation="nearest"):
     """FP16 kCHW2 image [ceil(C/2), H, W, 2] (rotate_h2, rotateKernel.h:18-20). Returns kCHW2."""
-    assert img_chw2.is_cuda and img_chw2.dtype == torch.float16 and img_chw2.shape[-1] == 2
-    img_chw2 = img_chw2.contiguous()
+    img_chw2 = _check_packed("rotate_chw2", img_chw2, channels, 2, torch.float16)
     _, h, w, _ = img_chw2.shape
     angle, center = _scalars(img_chw2, angle, center, torch.float16)
     out = torch.empty_like(img_chw2)
@@ -123,8 +133,7 @@ def rotate_chw2(img_chw2, channels, angle, center, interpolation="nearest"):
 def rotate_int8(img_chw4, scale_i, channels, angle, center, scale_o, interpolation="nearest"):
     """INT8 kCHW4 image [ceil(C/4), H, W, 4] with per-tensor scales (real = q*scale); angle / center float32 or
     float16 tensors (rotate_int8<T>, rotateKernel.h:22-26; rotatePlugin.cpp:101-111). Returns kCHW4 int8."""
-    assert img_chw4.is_cuda and img_chw4.dtype == torch.int8 and img_chw4.shape[-1] == 4
-    img_chw4 = img_chw4.contiguous()
+    img_chw4 = _check_packed("rotate_int8", img_chw4, channels, 4, torch.int8)
     _, h, w, _ = img_chw4.shape
     adt = angle.dtype if torch.is_tensor(angle) and angle.dtype == torch.float16 else torch.float32
     angle, center = _scalars(img_chw4, angle, center, adt)

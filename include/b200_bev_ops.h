@@ -651,12 +651,24 @@ int b200_dcn_f16_chw2(const void *input, const void *weight, const void *bias, c
  * attributes), so that a TensorRT shell — or a test — forwards verbatim, as b200_msda_enqueue does for MSDA.
  * ---------------------------------------------------------------------------------------------------------- */
 /* GridSampler{2D,3D}TRT[2] (gridSamplerPlugin.cpp:110-155): inputs = input, grid; dispatch on the input descriptor's
- * type / format (fp32, fp16 linear, fp16 kCHW2, int8 kCHW4 with the descriptors' scales). Needs no workspace. */
+ * type / format (fp32, fp16 linear, fp16 kCHW2, int8 kCHW4 with the descriptors' scales). The grid and output
+ * descriptors must have the input's rank and the output dims must be [N, C, grid spatial], else B200_ERR_BAD_PARAM.
+ * Needs no workspace. */
 int b200_grid_sampler_enqueue(const b200_tensor_desc *input_desc, const b200_tensor_desc *output_desc,
                               const void *const *inputs, void *const *outputs, void *workspace, void *stream,
                               int interpolation_mode, int padding_mode, int align_corners);
 /* supportsFormatCombination mirror (gridSamplerPlugin.cpp:168-194): in_out = {input, grid, output}. */
 int b200_grid_sampler_supports_format(int pos, const b200_tensor_desc *in_out, int nb_inputs, int nb_outputs, int use_h2);
+
+/* RotateTRT[2] (rotatePlugin.cpp:75-113): inputs = img [C, H, W], angle [1], center [2]; interp = the plugin attribute,
+ * use_h2 = the …TRT2 flavour (FP16 as kCHW2 packets). B200_ERR_BAD_PARAM unless img has rank 3, the output dims equal
+ * img's, angle has 1 element and center 2. Dispatch on img's type: fp32, fp16, int8 kCHW4 with the descriptors' scales
+ * (angle / center __half when the angle descriptor is kHALF). Needs no workspace. */
+int b200_rotate_enqueue(const b200_tensor_desc *input_desc, const b200_tensor_desc *output_desc,
+                        const void *const *inputs, void *const *outputs, void *workspace, void *stream, int interp,
+                        int use_h2);
+/* supportsFormatCombination mirror (rotatePlugin.cpp:122-153): in_out = {img, angle, center, output}. */
+int b200_rotate_supports_format(int pos, const b200_tensor_desc *in_out, int nb_inputs, int nb_outputs, int use_h2);
 
 /* ModulatedDeformableConv2dTRT[2] (…Conv2dPlugin.cpp:117-199): inputs = x, offset, mask, weight[, bias] (nb_inputs 4 or
  * 5). stride / padding / dilation = the plugin attributes' int[2] in ONNX order (h, w), as the exporter writes them
@@ -670,6 +682,10 @@ size_t b200_dcn_enqueue_workspace_size(const b200_tensor_desc *input_desc, const
 int b200_dcn_enqueue(const b200_tensor_desc *input_desc, const b200_tensor_desc *output_desc, const void *const *inputs,
                      void *const *outputs, void *workspace, void *stream, int nb_inputs, const int32_t *stride,
                      const int32_t *padding, const int32_t *dilation, int groups, int deform_groups);
+/* supportsFormatCombination mirror (…Conv2dPlugin.cpp:213-250): in_out = {x, offset, mask, weight[, bias], output};
+ * groups = the plugin attribute (INT8 needs C and Co / groups to be multiples of 4). */
+int b200_dcn_supports_format(int pos, const b200_tensor_desc *in_out, int nb_inputs, int nb_outputs, int groups,
+                             int use_h2);
 
 /* ------------------------------------------------------------------------------------------------------------
  * BEVPoolV2 (plugins BEVPoolV2TRT / BEVPoolV2TRT2; TensorRT/plugin/bev_pool_v2/bevPoolKernel.h, backward
