@@ -1,7 +1,7 @@
 """oracle/f64.py — TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
-Float64 references of multi-scale deformable attention and DCNv2, forward and backward, written from the definition of
-each op in plain torch. Every output and gradient element ``e`` comes with what a per-element rounding bound needs:
+Float64 references of multi-scale deformable attention and DCNv2, forward and backward, and of rotate's sampling step,
+written from the definition of each op in plain torch. Every output and gradient element ``e`` comes with what a per-element rounding bound needs:
 
 * ``r``    its value;
 * ``mag``  the sum of |terms| that make up ``r`` (the same computation on magnitudes where the op is monotone; written out
@@ -284,3 +284,36 @@ def dcn_f64(x, offset, mask, weight, bias, stride=1, padding=0, dilation=1, grou
     res["grad_input"] = _entry(gi.reshape(N, C, H, W), gia.reshape(N, C, H, W),
                                (cnt + Mg + 9).expand(N, dg, cpd, H * W).reshape(N, C, H, W))
     return res
+
+
+def rotate_f64(img, ix, iy, interp):
+    """RotateTRT's sampling step: img [C, H, W] (the values the kernel reads: FP16 values widened, or the fp32 products
+    q * scale_i for INT8), ix / iy [H, W] the source index of every output pixel (float32, as the kernel forms them).
+    Bilinear (interp 0): the four taps around (ix, iy) weighted (x1 - ix)(y1 - iy), (ix - x0)(y1 - iy),
+    (x1 - ix)(iy - y0), (ix - x0)(iy - y0) in float64, a tap outside the image contributing 0; n = 4. Nearest
+    (interp 1): the pixel at round-half-away-from-zero (ix, iy) (roundf), 0 outside; n = 1. Same entry as above, on the
+    device of ``img``; mag = sum |w_i v_i|."""
+    v = img.detach().to(F64)
+    C, H, W = v.shape
+    flat = v.reshape(C, H * W)
+    x, y = ix.detach().to(v.device, F64), iy.detach().to(v.device, F64)
+
+    def tap(xi, yi):
+        ok = (xi >= 0) & (xi < W) & (yi >= 0) & (yi < H)
+        pix = (yi.clamp(0, H - 1) * W + xi.clamp(0, W - 1)).long().reshape(-1)
+        return flat[:, pix].reshape(C, H, W) * ok
+
+    if interp == 1:
+        rnd = lambda t: torch.sign(t) * torch.floor(t.abs() + 0.5)  # noqa: E731
+        r = tap(rnd(x), rnd(y))
+        return _entry(r, r.abs(), 1)
+    x0, y0 = x.floor(), y.floor()
+    x1, y1 = x0 + 1, y0 + 1
+    r = torch.zeros(C, H, W, dtype=F64, device=v.device)
+    mag = torch.zeros_like(r)
+    for xi, yi, w in ((x0, y0, (x1 - x) * (y1 - y)), (x1, y0, (x - x0) * (y1 - y)), (x0, y1, (x1 - x) * (y - y0)),
+                      (x1, y1, (x - x0) * (y - y0))):  # fmt: skip
+        t = tap(xi, yi) * w
+        r += t
+        mag += t.abs()
+    return _entry(r, mag, 4)

@@ -56,14 +56,10 @@ import bevformer_tensorrt_b200 as bt
 from oracle import dcn as odcn
 from oracle import msda as omsda
 from oracle.f64 import dcn_f64, msda_f64, msda_sca_f64
-from tests.helpers import kernels_recorded
+from tests.helpers import U32, check, kernels_recorded, ulp
 from tests.test_dcn_backward_edges_gpu import _plan, _ragged, _ws_query
 
-U32 = 2.0**-24
-U_DTYPE = {torch.float32: 2.0**-24, torch.float16: 2.0**-11, torch.bfloat16: 2.0**-8}
-S_DTYPE = {torch.float32: 2.0**-150, torch.float16: 2.0**-25, torch.bfloat16: 2.0**-134}  # half the least subnormal
 U_WGMMA = 2.0**-23
-_MANT = {torch.float32: (23, -126), torch.float16: (10, -14), torch.bfloat16: (7, -126)}
 DTYPES = [torch.float32, torch.float16, torch.bfloat16]
 DT_IDS = ["fp32", "fp16", "bf16"]
 
@@ -73,53 +69,6 @@ DCN_SEEDS = [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 13, 26, 66, 490, 651, 940]
 _EXTRA = int(os.environ.get("B200_SWEEP_SEEDS", "0") or 0)
 MSDA_SEEDS += [100_000 + i for i in range(_EXTRA)]
 DCN_SEEDS += [100_000 + i for i in range(_EXTRA)]
-
-
-# ---- the bound ---------------------------------------------------------------------------------------------------------
-def ulp(a, dtype):
-    """Spacing of ``dtype`` at the float64 magnitudes ``a`` (subnormal spacing below the smallest normal)."""
-    mant, emin = _MANT[dtype]
-    _, e = torch.frexp(a)
-    return torch.ldexp(torch.ones_like(a), torch.clamp(e - 1, min=emin) - mant)
-
-
-def element_bound(ent, u_acc, dtype, low=None):
-    """``low``: the dtype the path rounds intermediates to, or None."""
-    E = (8 + ent["n"]) * u_acc * ent["mag"] + U32 * ent["pmag"]
-    if low is not None:
-        E = E + U_DTYPE[low] * ent["lmag"] + S_DTYPE[low] * ent["lcnt"]
-    return 0.5 * ulp(ent["r"].abs() + E, dtype) + E
-
-
-def tensor_bar(r, dtype):
-    m = float(r.abs().max()) if r.numel() else 0.0
-    if dtype == torch.float32:
-        return 1e-4 * m
-    return 0.5 * float(ulp(torch.tensor([m], dtype=torch.float64), dtype)) + 1e-4 * m
-
-
-def check(tag, name, got, ent, u_acc, low=None, bar=None):
-    """Asserts the per-element bound on every element of ``got`` (and the per-tensor bar); reports the worst element."""
-    assert got is not None, f"{tag}: {name} was requested but is None"
-    r = ent["r"]
-    assert tuple(got.shape) == tuple(r.shape), (tag, name, tuple(got.shape), tuple(r.shape))
-    g = got.detach().to(r.device, torch.float64)
-    bound = element_bound(ent, u_acc, got.dtype, low)
-    err = (g - r).abs()
-    bad = ~(err <= bound)
-    if bool(bad.any()):
-        ratio = torch.where(bad, err / bound.clamp(min=1e-300), torch.zeros_like(err))
-        i = int(ratio.reshape(-1).argmax())
-        idx = np.unravel_index(i, tuple(r.shape))
-        raise AssertionError(f"{tag} {name}: {int(bad.sum())} of {r.numel()} elements outside the bound; worst at "
-                             f"{tuple(int(v) for v in idx)}: got {g.reshape(-1)[i].item()!r} ref {r.reshape(-1)[i].item()!r} "
-                             f"bound {bound.reshape(-1)[i].item():.3e} (mag {ent['mag'].reshape(-1)[i].item():.3e})")  # fmt: skip
-    if not r.numel():
-        return
-    b = tensor_bar(r, got.dtype) if bar is None else bar
-    if low is not None and bar is None:  # the largest intermediate rounding on top of the per-tensor bar
-        b += U_DTYPE[low] * float(ent["lmag"].max()) + S_DTYPE[low] * float(ent["lcnt"].max())
-    assert float(err.max()) <= b, (tag, name, float(err.max()), b)
 
 
 # ---- MSDA geometries ---------------------------------------------------------------------------------------------------
