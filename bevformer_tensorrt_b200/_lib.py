@@ -133,10 +133,14 @@ SIGNATURES = {
     # num_intervals, depth_size, feat_rows, out_height, out_width, out, stream
     "b200_bev_pool_f32": (_i, [_vp] * 7 + _BEV_POOL_DIMS + [_vp, _vp]),
     "b200_bev_pool_f16": (_i, [_vp] * 7 + _BEV_POOL_DIMS + [_vp, _vp]),
+    "b200_bev_pool_bf16": (_i, [_vp] * 7 + _BEV_POOL_DIMS + [_vp, _vp]),
+    "b200_bev_pool_f32_depth": (_i, [_i] + [_vp] * 7 + _BEV_POOL_DIMS + [_vp, _vp]),  # feat_dtype first
     "b200_bev_pool_i8": (_i, [_vp, _f, _vp, _f] + [_vp] * 5 + _BEV_POOL_DIMS + [_vp, _f, _vp]),
     "b200_bev_pool_backward_workspace_size": (ctypes.c_size_t, [_i]),
     "b200_bev_pool_backward_f32": (_i, [_vp] * 9 + _BEV_POOL_DIMS + [_vp, _vp, _vp, ctypes.c_size_t, _vp]),
     "b200_bev_pool_backward_f16": (_i, [_vp] * 9 + _BEV_POOL_DIMS + [_vp, _vp, _vp, ctypes.c_size_t, _vp]),
+    "b200_bev_pool_backward_bf16": (_i, [_vp] * 9 + _BEV_POOL_DIMS + [_vp, _vp, _vp, ctypes.c_size_t, _vp]),
+    "b200_bev_pool_backward_f32_depth": (_i, [_i] + [_vp] * 9 + _BEV_POOL_DIMS + [_vp, _vp, _vp, ctypes.c_size_t, _vp]),
     "b200_bev_pool_enqueue": (_i, [ctypes.POINTER(TensorDesc), ctypes.POINTER(TensorDesc), ctypes.POINTER(_vp),
                                    ctypes.POINTER(_vp), _vp, _vp, _i, _i]),
     "b200_bev_pool_supports_format": (_i, [_i, ctypes.POINTER(TensorDesc), _i, _i]),

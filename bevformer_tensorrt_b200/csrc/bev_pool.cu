@@ -1,5 +1,6 @@
-// bev_pool.cu — BEVPoolV2 (plugins BEVPoolV2TRT / BEVPoolV2TRT2) on sm_90a: forward in FP32 / FP16 / INT8 and the
-// depth / feature gradients in FP32 / FP16.
+// bev_pool.cu — BEVPoolV2 (plugins BEVPoolV2TRT / BEVPoolV2TRT2) on sm_90a: forward in FP32 / FP16 / BF16 / INT8 and
+// the depth / feature gradients in FP32 / FP16 / BF16, and FP32 depth with FP16 / BF16 features (what torch.autocast
+// hands the op: a softmax depth and conv features), forward and both gradients.
 //
 // For every interval k (s = interval_starts[k], len = interval_lengths[k], cell = ranks_bev[s]):
 //   out[cell, c] = sum_{i = s}^{s + len - 1} feat[ranks_feat[i], c] * depth[ranks_depth[i]]
@@ -16,6 +17,11 @@
 // at a time, coalesced and evict-first, and hands them out by shuffle; four feat rows are in flight per lane. Each lane
 // keeps one accumulator per channel and adds the points in their order: FP32 is the reference kernel's FFMA chain bit
 // for bit, FP16 accumulates in FP32 and rounds once, INT8 sums exactly in int32 and requantises as the reference does.
+// BF16 is FP16's arithmetic on bf16 storage (each element widened exactly, `u << 16`). FP32 depth (depth element type TD
+// = float, features T = FP16 / BF16) changes three things only: the per-point depth load of the forward and of the
+// feature gradient, and the depth-gradient store, which is not rounded. Those instantiations have __global__ wrappers
+// of their own (bev_pool*_f32_depth_kernel) around the same __device__ body, so the same-dtype kernels keep their
+// names and templates <T, VEC>.
 #include <type_traits>
 
 #include "common.cuh"
@@ -25,6 +31,8 @@ namespace b200 {
 namespace {
 
 constexpr int kBevThreads = 256;
+// feat_dtype of the FP32-depth entries: nvinfer1::DataType's codes, as the MSDA / DCN workspace queries take them
+constexpr int kFeatF16 = 1, kFeatBF16 = 7;
 
 struct BevPoolArgs {
   const int32_t *ranks_depth, *ranks_feat, *ranks_bev, *starts, *lengths;
@@ -43,16 +51,19 @@ using AccT = typename std::conditional<std::is_same<T, int8_t>::value, int, floa
 template <typename T>
 __device__ __forceinline__ AccT<T> widen(T x) {
   if constexpr (std::is_same<T, __half>::value) return __half2float(x);
+  else if constexpr (std::is_same<T, __nv_bfloat16>::value) return bf16_to_f(x);
   else return static_cast<AccT<T>>(x);
 }
 
 template <typename T>
 __device__ __forceinline__ T narrow(float x) {
   if constexpr (std::is_same<T, __half>::value) return __float2half_rn(x);
+  else if constexpr (std::is_same<T, __nv_bfloat16>::value) return __float2bfloat16_rn(x);
   else return x;
 }
 
-// acc + f * d: one FFMA for FP32 and FP16 (the product of two halves is exact in FP32), an exact int32 MAD for INT8
+// acc + f * d: one FFMA for FP32, FP16 and BF16 (the product of two 2-byte values is exact in FP32), an exact int32 MAD
+// for INT8
 template <typename T>
 __device__ __forceinline__ AccT<T> mad(T f, AccT<T> d, AccT<T> acc) {
   if constexpr (std::is_same<T, int8_t>::value) return acc + static_cast<int>(f) * d;
@@ -79,10 +90,9 @@ __device__ __forceinline__ unsigned group_mask(int G) {
   return G == 32 ? kFullMask : ((1u << G) - 1) << ((threadIdx.x & 31) & ~(G - 1));
 }
 
-template <typename T, int VEC>
-__global__ void __launch_bounds__(kBevThreads) bev_pool_kernel(const BevPoolArgs a, const T *__restrict__ depth,
-                                                               const T *__restrict__ feat, T *__restrict__ out,
-                                                               float scale_io, int G) {
+template <typename T, typename TD, int VEC>
+__device__ __forceinline__ void bev_pool_body(const BevPoolArgs a, const TD *__restrict__ depth,
+                                              const T *__restrict__ feat, T *__restrict__ out, float scale_io, int G) {
   using Acc = AccT<T>;
   using P = Pack<T, VEC>;
   const int gl = threadIdx.x & (G - 1);
@@ -137,14 +147,28 @@ __global__ void __launch_bounds__(kBevThreads) bev_pool_kernel(const BevPoolArgs
   *reinterpret_cast<P *>(out + static_cast<size_t>(cell) * a.C + c0) = o;
 }
 
+template <typename T, int VEC>
+__global__ void __launch_bounds__(kBevThreads) bev_pool_kernel(const BevPoolArgs a, const T *__restrict__ depth,
+                                                               const T *__restrict__ feat, T *__restrict__ out,
+                                                               float scale_io, int G) {
+  bev_pool_body<T, T, VEC>(a, depth, feat, out, scale_io, G);
+}
+
+template <typename T, int VEC>
+__global__ void __launch_bounds__(kBevThreads) bev_pool_f32_depth_kernel(const BevPoolArgs a,
+                                                                         const float *__restrict__ depth,
+                                                                         const T *__restrict__ feat,
+                                                                         T *__restrict__ out, int G) {
+  bev_pool_body<T, float, VEC>(a, depth, feat, out, 0.f, G);
+}
+
 // Backward, step 1 (one group per interval): depth_grad[rd] = sum_c out_grad[cell, c] * feat[rf, c] for every kept point
 // (a fixed-order lane-partial FFMA chain and butterfly sum), and point_cell[i] = the cell point i pooled into, -1 when it
 // pooled into none. With depth_grad == NULL only point_cell is written.
-template <typename T, int VEC>
-__global__ void __launch_bounds__(kBevThreads) bev_pool_depth_grad_kernel(const BevPoolArgs a, const T *__restrict__ out_grad,
-                                                                          const T *__restrict__ feat,
-                                                                          T *__restrict__ depth_grad,
-                                                                          int *__restrict__ point_cell, int G) {
+template <typename T, typename TD, int VEC>
+__device__ __forceinline__ void bev_pool_depth_grad_body(const BevPoolArgs a, const T *__restrict__ out_grad,
+                                                         const T *__restrict__ feat, TD *__restrict__ depth_grad,
+                                                         int *__restrict__ point_cell, int G) {
   using P = Pack<T, VEC>;
   const int gl = threadIdx.x & (G - 1);
   const long long k = group_index(G);
@@ -174,19 +198,35 @@ __global__ void __launch_bounds__(kBevThreads) bev_pool_depth_grad_kernel(const 
         for (int v = 0; v < VEC; ++v) part = __fmaf_rn(widen(g.v[v]), widen(x.v[v]), part);
       }
       for (int o = G / 2; o > 0; o >>= 1) part = __fadd_rn(part, __shfl_xor_sync(mask, part, o, G));
-      if (gl == 0) depth_grad[rdj] = narrow<T>(part);
+      if (gl == 0) depth_grad[rdj] = narrow<TD>(part);
     }
   }
 }
 
+template <typename T, int VEC>
+__global__ void __launch_bounds__(kBevThreads) bev_pool_depth_grad_kernel(const BevPoolArgs a, const T *__restrict__ out_grad,
+                                                                          const T *__restrict__ feat,
+                                                                          T *__restrict__ depth_grad,
+                                                                          int *__restrict__ point_cell, int G) {
+  bev_pool_depth_grad_body<T, T, VEC>(a, out_grad, feat, depth_grad, point_cell, G);
+}
+
+template <typename T, int VEC>
+__global__ void __launch_bounds__(kBevThreads) bev_pool_depth_grad_f32_depth_kernel(const BevPoolArgs a,
+                                                                                    const T *__restrict__ out_grad,
+                                                                                    const T *__restrict__ feat,
+                                                                                    float *__restrict__ depth_grad,
+                                                                                    int *__restrict__ point_cell, int G) {
+  bev_pool_depth_grad_body<T, float, VEC>(a, out_grad, feat, depth_grad, point_cell, G);
+}
+
 // Backward, step 2 (one group per run of equal ranks_feat in `order`, the points sorted by ranks_feat):
 // feat_grad[rf, c] = sum over the run's pooled points of out_grad[cell, c] * depth[rd], in run order.
-template <typename T, int VEC>
-__global__ void __launch_bounds__(kBevThreads) bev_pool_feat_grad_kernel(const BevPoolArgs a, const int32_t *__restrict__ order,
-                                                                         const T *__restrict__ out_grad,
-                                                                         const T *__restrict__ depth,
-                                                                         const int *__restrict__ point_cell,
-                                                                         T *__restrict__ feat_grad, int G) {
+template <typename T, typename TD, int VEC>
+__device__ __forceinline__ void bev_pool_feat_grad_body(const BevPoolArgs a, const int32_t *__restrict__ order,
+                                                        const T *__restrict__ out_grad, const TD *__restrict__ depth,
+                                                        const int *__restrict__ point_cell, T *__restrict__ feat_grad,
+                                                        int G) {
   using P = Pack<T, VEC>;
   const int gl = threadIdx.x & (G - 1);
   const long long jl = group_index(G);
@@ -221,6 +261,25 @@ __global__ void __launch_bounds__(kBevThreads) bev_pool_feat_grad_kernel(const B
   *reinterpret_cast<P *>(feat_grad + static_cast<size_t>(rf) * a.C + c0) = o;
 }
 
+template <typename T, int VEC>
+__global__ void __launch_bounds__(kBevThreads) bev_pool_feat_grad_kernel(const BevPoolArgs a, const int32_t *__restrict__ order,
+                                                                         const T *__restrict__ out_grad,
+                                                                         const T *__restrict__ depth,
+                                                                         const int *__restrict__ point_cell,
+                                                                         T *__restrict__ feat_grad, int G) {
+  bev_pool_feat_grad_body<T, T, VEC>(a, order, out_grad, depth, point_cell, feat_grad, G);
+}
+
+template <typename T, int VEC>
+__global__ void __launch_bounds__(kBevThreads) bev_pool_feat_grad_f32_depth_kernel(const BevPoolArgs a,
+                                                                                   const int32_t *__restrict__ order,
+                                                                                   const T *__restrict__ out_grad,
+                                                                                   const float *__restrict__ depth,
+                                                                                   const int *__restrict__ point_cell,
+                                                                                   T *__restrict__ feat_grad, int G) {
+  bev_pool_feat_grad_body<T, float, VEC>(a, order, out_grad, depth, point_cell, feat_grad, G);
+}
+
 // Widest vector (elements) that divides C and keeps every row of every listed tensor aligned.
 template <typename T>
 int pick_vec(int C, std::initializer_list<const void *> ptrs) {
@@ -247,93 +306,108 @@ dim3 grid_of(long long items, int C, int vec, int G, bool tiled) {
 
 bool aligned(const void *p, size_t bytes) { return reinterpret_cast<uintptr_t>(p) % bytes == 0; }
 
-// elem: the byte size of a depth / feat / out element. Every pointer must be aligned to its element.
+// depth_elem: the byte size of a depth element (and of the depth gradient's); elem: that of a feat / out element (and
+// of out_grad's and the feature gradient's). Every pointer must be aligned to its element.
 int check_args(const void *depth, const void *feat, const void *out, const int32_t *rd, const int32_t *rf,
                const int32_t *rb, const int32_t *st, const int32_t *ln, int C, int P, int I, long long depth_size,
-               long long feat_rows, int out_h, int out_w, size_t elem) {
+               long long feat_rows, int out_h, int out_w, size_t depth_elem, size_t elem) {
   if (C <= 0 || P < 0 || I < 0 || depth_size < 0 || feat_rows < 0 || out_h <= 0 || out_w <= 0) return B200_ERR_BAD_PARAM;
   if (!out || (P > 0 && (!rd || !rf || !rb)) || (I > 0 && (!st || !ln))) return B200_ERR_BAD_PARAM;
   if ((depth_size > 0 && !depth) || (feat_rows > 0 && !feat)) return B200_ERR_BAD_PARAM;
   if (feat_rows > (1ll << 62) / C) return B200_ERR_BAD_PARAM;
-  for (const void *p : {depth, feat, out})
+  if (!aligned(depth, depth_elem)) return B200_ERR_BAD_PARAM;
+  for (const void *p : {feat, out})
     if (!aligned(p, elem)) return B200_ERR_BAD_PARAM;
   for (const int32_t *p : {rd, rf, rb, st, ln})
     if (!aligned(p, sizeof(int32_t))) return B200_ERR_BAD_PARAM;
   return B200_OK;
 }
 
-template <typename T, int VEC>
-void launch_fwd(const BevPoolArgs &a, const T *depth, const T *feat, T *out, float scale_io, cudaStream_t s) {
+template <typename T, typename TD, int VEC>
+void launch_fwd(const BevPoolArgs &a, const TD *depth, const T *feat, T *out, float scale_io, cudaStream_t s) {
   const int G = group_size(a.C, VEC);
-  bev_pool_kernel<T, VEC><<<grid_of(a.I, a.C, VEC, G, true), kBevThreads, 0, s>>>(a, depth, feat, out, scale_io, G);
+  const dim3 grid = grid_of(a.I, a.C, VEC, G, true);
+  if constexpr (std::is_same<T, TD>::value)
+    bev_pool_kernel<T, VEC><<<grid, kBevThreads, 0, s>>>(a, depth, feat, out, scale_io, G);
+  else
+    bev_pool_f32_depth_kernel<T, VEC><<<grid, kBevThreads, 0, s>>>(a, depth, feat, out, G);
 }
 
-template <typename T>
-int bev_pool_forward(const BevPoolArgs &a, const T *depth, const T *feat, T *out, float scale_io, void *stream) {
+template <typename T, typename TD = T>
+int bev_pool_forward(const BevPoolArgs &a, const TD *depth, const T *feat, T *out, float scale_io, void *stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (cudaMemsetAsync(out, 0, static_cast<size_t>(a.cells) * a.C * sizeof(T), s) != cudaSuccess) return B200_ERR_LAUNCH;
   if (a.I == 0) return B200_OK;
   switch (pick_vec<T>(a.C, {feat, out})) {
-    case 16: if constexpr (sizeof(T) == 1) launch_fwd<T, 16>(a, depth, feat, out, scale_io, s); break;
-    case 8: if constexpr (sizeof(T) <= 2) launch_fwd<T, 8>(a, depth, feat, out, scale_io, s); break;
-    case 4: launch_fwd<T, 4>(a, depth, feat, out, scale_io, s); break;
-    case 2: launch_fwd<T, 2>(a, depth, feat, out, scale_io, s); break;
-    default: launch_fwd<T, 1>(a, depth, feat, out, scale_io, s); break;
+    case 16: if constexpr (sizeof(T) == 1) launch_fwd<T, TD, 16>(a, depth, feat, out, scale_io, s); break;
+    case 8: if constexpr (sizeof(T) <= 2) launch_fwd<T, TD, 8>(a, depth, feat, out, scale_io, s); break;
+    case 4: launch_fwd<T, TD, 4>(a, depth, feat, out, scale_io, s); break;
+    case 2: launch_fwd<T, TD, 2>(a, depth, feat, out, scale_io, s); break;
+    default: launch_fwd<T, TD, 1>(a, depth, feat, out, scale_io, s); break;
   }
   return check_launch();
 }
 
-template <typename T, int VEC>
-void launch_depth_grad(const BevPoolArgs &a, const T *out_grad, const T *feat, T *depth_grad, int *point_cell,
+template <typename T, typename TD, int VEC>
+void launch_depth_grad(const BevPoolArgs &a, const T *out_grad, const T *feat, TD *depth_grad, int *point_cell,
                        cudaStream_t s) {
   const int G = group_size(a.C, VEC);
-  bev_pool_depth_grad_kernel<T, VEC><<<grid_of(a.I, a.C, VEC, G, false), kBevThreads, 0, s>>>(a, out_grad, feat,
-                                                                                              depth_grad, point_cell, G);
+  const dim3 grid = grid_of(a.I, a.C, VEC, G, false);
+  if constexpr (std::is_same<T, TD>::value)
+    bev_pool_depth_grad_kernel<T, VEC><<<grid, kBevThreads, 0, s>>>(a, out_grad, feat, depth_grad, point_cell, G);
+  else
+    bev_pool_depth_grad_f32_depth_kernel<T, VEC><<<grid, kBevThreads, 0, s>>>(a, out_grad, feat, depth_grad,
+                                                                              point_cell, G);
 }
 
-template <typename T, int VEC>
-void launch_feat_grad(const BevPoolArgs &a, const int32_t *order, const T *out_grad, const T *depth,
+template <typename T, typename TD, int VEC>
+void launch_feat_grad(const BevPoolArgs &a, const int32_t *order, const T *out_grad, const TD *depth,
                       const int *point_cell, T *feat_grad, cudaStream_t s) {
   const int G = group_size(a.C, VEC);
-  bev_pool_feat_grad_kernel<T, VEC><<<grid_of(a.P, a.C, VEC, G, true), kBevThreads, 0, s>>>(a, order, out_grad, depth,
-                                                                                           point_cell, feat_grad, G);
+  const dim3 grid = grid_of(a.P, a.C, VEC, G, true);
+  if constexpr (std::is_same<T, TD>::value)
+    bev_pool_feat_grad_kernel<T, VEC><<<grid, kBevThreads, 0, s>>>(a, order, out_grad, depth, point_cell, feat_grad, G);
+  else
+    bev_pool_feat_grad_f32_depth_kernel<T, VEC><<<grid, kBevThreads, 0, s>>>(a, order, out_grad, depth, point_cell,
+                                                                             feat_grad, G);
 }
 
 // Each kernel takes its vector width from the tensors it reads and writes alone, so the depth gradient's lane partition,
-// and with it its bits, does not depend on whether or where a feature gradient is asked for.
-template <typename T>
-int bev_pool_backward(const BevPoolArgs &a, const int32_t *order, const T *out_grad, const T *depth, const T *feat,
-                      T *depth_grad, T *feat_grad, void *workspace, size_t workspace_size, void *stream) {
+// and with it its bits, does not depend on whether or where a feature gradient is asked for. The depth tensors (TD)
+// are read or written one element per point and never set the width.
+template <typename T, typename TD = T>
+int bev_pool_backward(const BevPoolArgs &a, const int32_t *order, const T *out_grad, const TD *depth, const T *feat,
+                      TD *depth_grad, T *feat_grad, void *workspace, size_t workspace_size, void *stream) {
   if (!out_grad || (!depth_grad && !feat_grad)) return B200_ERR_BAD_PARAM;
   if (feat_grad && a.P > 0 && !order) return B200_ERR_BAD_PARAM;
-  if (!aligned(depth_grad, sizeof(T)) || !aligned(feat_grad, sizeof(T)) || !aligned(order, sizeof(int32_t)) ||
+  if (!aligned(depth_grad, sizeof(TD)) || !aligned(feat_grad, sizeof(T)) || !aligned(order, sizeof(int32_t)) ||
       !aligned(workspace, sizeof(int)))
     return B200_ERR_BAD_PARAM;
   const size_t ws = b200_bev_pool_backward_workspace_size(a.P);
   if (ws && (!workspace || workspace_size < ws)) return B200_ERR_BAD_PARAM;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int *point_cell = static_cast<int *>(workspace);
-  if (depth_grad && cudaMemsetAsync(depth_grad, 0, static_cast<size_t>(a.depth_size) * sizeof(T), s) != cudaSuccess)
+  if (depth_grad && cudaMemsetAsync(depth_grad, 0, static_cast<size_t>(a.depth_size) * sizeof(TD), s) != cudaSuccess)
     return B200_ERR_LAUNCH;
   if (feat_grad && cudaMemsetAsync(feat_grad, 0, static_cast<size_t>(a.feat_rows) * a.C * sizeof(T), s) != cudaSuccess)
     return B200_ERR_LAUNCH;
   if (ws && cudaMemsetAsync(point_cell, 0xff, ws, s) != cudaSuccess) return B200_ERR_LAUNCH;
   if (a.I > 0) {
     switch (pick_vec<T>(a.C, {out_grad, feat})) {
-      case 8: if constexpr (sizeof(T) <= 2) launch_depth_grad<T, 8>(a, out_grad, feat, depth_grad, point_cell, s); break;
-      case 4: launch_depth_grad<T, 4>(a, out_grad, feat, depth_grad, point_cell, s); break;
-      case 2: launch_depth_grad<T, 2>(a, out_grad, feat, depth_grad, point_cell, s); break;
-      default: launch_depth_grad<T, 1>(a, out_grad, feat, depth_grad, point_cell, s); break;
+      case 8: if constexpr (sizeof(T) <= 2) launch_depth_grad<T, TD, 8>(a, out_grad, feat, depth_grad, point_cell, s); break;
+      case 4: launch_depth_grad<T, TD, 4>(a, out_grad, feat, depth_grad, point_cell, s); break;
+      case 2: launch_depth_grad<T, TD, 2>(a, out_grad, feat, depth_grad, point_cell, s); break;
+      default: launch_depth_grad<T, TD, 1>(a, out_grad, feat, depth_grad, point_cell, s); break;
     }
     const int st = check_launch();
     if (st != B200_OK) return st;
   }
   if (!feat_grad || a.P == 0) return B200_OK;
   switch (pick_vec<T>(a.C, {out_grad, feat_grad})) {
-    case 8: if constexpr (sizeof(T) <= 2) launch_feat_grad<T, 8>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
-    case 4: launch_feat_grad<T, 4>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
-    case 2: launch_feat_grad<T, 2>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
-    default: launch_feat_grad<T, 1>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
+    case 8: if constexpr (sizeof(T) <= 2) launch_feat_grad<T, TD, 8>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
+    case 4: launch_feat_grad<T, TD, 4>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
+    case 2: launch_feat_grad<T, TD, 2>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
+    default: launch_feat_grad<T, TD, 1>(a, order, out_grad, depth, point_cell, feat_grad, s); break;
   }
   return check_launch();
 }
@@ -356,7 +430,7 @@ int b200_bev_pool_f32(const float *depth, const float *feat, const int32_t *rank
                       int out_height, int out_width, float *out, void *stream) {
   const int st = check_args(depth, feat, out, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths,
                             channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width,
-                            sizeof(float));
+                            sizeof(float), sizeof(float));
   if (st != B200_OK) return st;
   B200_BEV_POOL_ARGS;
   return bev_pool_forward<float>(a, depth, feat, out, 0.f, stream);
@@ -368,11 +442,43 @@ int b200_bev_pool_f16(const void *depth, const void *feat, const int32_t *ranks_
                       int out_height, int out_width, void *out, void *stream) {
   const int st = check_args(depth, feat, out, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths,
                             channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width,
-                            sizeof(__half));
+                            sizeof(__half), sizeof(__half));
   if (st != B200_OK) return st;
   B200_BEV_POOL_ARGS;
   return bev_pool_forward<__half>(a, static_cast<const __half *>(depth), static_cast<const __half *>(feat),
                                   static_cast<__half *>(out), 0.f, stream);
+}
+
+int b200_bev_pool_bf16(const void *depth, const void *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
+                       const int32_t *ranks_bev, const int32_t *interval_starts, const int32_t *interval_lengths,
+                       int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
+                       int out_height, int out_width, void *out, void *stream) {
+  const int st = check_args(depth, feat, out, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths,
+                            channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width,
+                            sizeof(__nv_bfloat16), sizeof(__nv_bfloat16));
+  if (st != B200_OK) return st;
+  B200_BEV_POOL_ARGS;
+  return bev_pool_forward<__nv_bfloat16>(a, static_cast<const __nv_bfloat16 *>(depth),
+                                         static_cast<const __nv_bfloat16 *>(feat), static_cast<__nv_bfloat16 *>(out),
+                                         0.f, stream);
+}
+
+int b200_bev_pool_f32_depth(int feat_dtype, const float *depth, const void *feat, const int32_t *ranks_depth,
+                            const int32_t *ranks_feat, const int32_t *ranks_bev, const int32_t *interval_starts,
+                            const int32_t *interval_lengths, int channels, int num_points, int num_intervals,
+                            int64_t depth_size, int64_t feat_rows, int out_height, int out_width, void *out,
+                            void *stream) {
+  if (feat_dtype != kFeatF16 && feat_dtype != kFeatBF16) return B200_ERR_UNSUPPORTED;
+  const int st = check_args(depth, feat, out, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths,
+                            channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width,
+                            sizeof(float), 2);
+  if (st != B200_OK) return st;
+  B200_BEV_POOL_ARGS;
+  if (feat_dtype == kFeatF16)
+    return bev_pool_forward<__half, float>(a, depth, static_cast<const __half *>(feat), static_cast<__half *>(out), 0.f,
+                                           stream);
+  return bev_pool_forward<__nv_bfloat16, float>(a, depth, static_cast<const __nv_bfloat16 *>(feat),
+                                                static_cast<__nv_bfloat16 *>(out), 0.f, stream);
 }
 
 int b200_bev_pool_i8(const int8_t *depth, float scale_depth, const int8_t *feat, float scale_feat,
@@ -382,7 +488,7 @@ int b200_bev_pool_i8(const int8_t *depth, float scale_depth, const int8_t *feat,
                      int8_t *out, float scale_out, void *stream) {
   const int st = check_args(depth, feat, out, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths,
                             channels, num_points, num_intervals, depth_size, feat_rows, out_height, out_width,
-                            sizeof(int8_t));
+                            sizeof(int8_t), sizeof(int8_t));
   if (st != B200_OK) return st;
   if (channels % 4 != 0) return B200_ERR_UNSUPPORTED;
   B200_BEV_POOL_ARGS;
@@ -402,7 +508,7 @@ int b200_bev_pool_backward_f32(const float *out_grad, const float *depth, const 
                                void *stream) {
   const int st = check_args(depth, feat, out_grad, ranks_depth, ranks_feat, ranks_bev, interval_starts,
                             interval_lengths, channels, num_points, num_intervals, depth_size, feat_rows, out_height,
-                            out_width, sizeof(float));
+                            out_width, sizeof(float), sizeof(float));
   if (st != B200_OK) return st;
   B200_BEV_POOL_ARGS;
   return bev_pool_backward<float>(a, feat_order, out_grad, depth, feat, depth_grad, feat_grad, workspace,
@@ -417,13 +523,53 @@ int b200_bev_pool_backward_f16(const void *out_grad, const void *depth, const vo
                                void *stream) {
   const int st = check_args(depth, feat, out_grad, ranks_depth, ranks_feat, ranks_bev, interval_starts,
                             interval_lengths, channels, num_points, num_intervals, depth_size, feat_rows, out_height,
-                            out_width, sizeof(__half));
+                            out_width, sizeof(__half), sizeof(__half));
   if (st != B200_OK) return st;
   B200_BEV_POOL_ARGS;
   return bev_pool_backward<__half>(a, feat_order, static_cast<const __half *>(out_grad),
                                    static_cast<const __half *>(depth), static_cast<const __half *>(feat),
                                    static_cast<__half *>(depth_grad), static_cast<__half *>(feat_grad), workspace,
                                    workspace_size, stream);
+}
+
+int b200_bev_pool_backward_bf16(const void *out_grad, const void *depth, const void *feat, const int32_t *ranks_depth,
+                                const int32_t *ranks_feat, const int32_t *ranks_bev, const int32_t *interval_starts,
+                                const int32_t *interval_lengths, const int32_t *feat_order, int channels,
+                                int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
+                                int out_height, int out_width, void *depth_grad, void *feat_grad, void *workspace,
+                                size_t workspace_size, void *stream) {
+  const int st = check_args(depth, feat, out_grad, ranks_depth, ranks_feat, ranks_bev, interval_starts,
+                            interval_lengths, channels, num_points, num_intervals, depth_size, feat_rows, out_height,
+                            out_width, sizeof(__nv_bfloat16), sizeof(__nv_bfloat16));
+  if (st != B200_OK) return st;
+  B200_BEV_POOL_ARGS;
+  using B = __nv_bfloat16;
+  return bev_pool_backward<B>(a, feat_order, static_cast<const B *>(out_grad), static_cast<const B *>(depth),
+                              static_cast<const B *>(feat), static_cast<B *>(depth_grad), static_cast<B *>(feat_grad),
+                              workspace, workspace_size, stream);
+}
+
+int b200_bev_pool_backward_f32_depth(int feat_dtype, const void *out_grad, const float *depth, const void *feat,
+                                     const int32_t *ranks_depth, const int32_t *ranks_feat, const int32_t *ranks_bev,
+                                     const int32_t *interval_starts, const int32_t *interval_lengths,
+                                     const int32_t *feat_order, int channels, int num_points, int num_intervals,
+                                     int64_t depth_size, int64_t feat_rows, int out_height, int out_width,
+                                     float *depth_grad, void *feat_grad, void *workspace, size_t workspace_size,
+                                     void *stream) {
+  if (feat_dtype != kFeatF16 && feat_dtype != kFeatBF16) return B200_ERR_UNSUPPORTED;
+  const int st = check_args(depth, feat, out_grad, ranks_depth, ranks_feat, ranks_bev, interval_starts,
+                            interval_lengths, channels, num_points, num_intervals, depth_size, feat_rows, out_height,
+                            out_width, sizeof(float), 2);
+  if (st != B200_OK) return st;
+  B200_BEV_POOL_ARGS;
+  if (feat_dtype == kFeatF16)
+    return bev_pool_backward<__half, float>(a, feat_order, static_cast<const __half *>(out_grad), depth,
+                                            static_cast<const __half *>(feat), depth_grad,
+                                            static_cast<__half *>(feat_grad), workspace, workspace_size, stream);
+  using B = __nv_bfloat16;
+  return bev_pool_backward<B, float>(a, feat_order, static_cast<const B *>(out_grad), depth,
+                                     static_cast<const B *>(feat), depth_grad, static_cast<B *>(feat_grad), workspace,
+                                     workspace_size, stream);
 }
 
 }  // extern "C"

@@ -12,13 +12,23 @@ the same cell, or a repeated ``ranks_depth``, are outside it. Every cell no inte
 every index is checked against the tensor it indexes: an interval whose cell is out of range is dropped, so is a point
 whose ``ranks_depth`` or ``ranks_feat`` is out of range, and ``[start, start + length)`` is clipped to ``[0, P)``.
 
-Index tensors go through ``.int()`` as in the reference (its TensorRT test feeds float ranks). The output has the
-input's dtype, as the plugin returns it; the reference's eager path returns float32 because mmdet3d's
-``QuickCumsumCuda`` upcasts. FP32 is the reference kernel's FFMA chain bit for bit; FP16 accumulates in FP32 and rounds
-once. Both names run the same kernels.
+Index tensors go through ``.int()`` as in the reference (its TensorRT test feeds float ranks). Dtypes (depth, feat):
 
-Trainable: the backward returns the depth and feature gradients in the input's dtype (FP32 accumulation, no atomics, the
-same bits on every run and for every subset of gradients). ``bev_pool_v2_int8`` is the INT8 inference form.
+    depth     feat      out       depth grad   feat grad
+    float32   float32   float32   float32      float32
+    float16   float16   float16   float16      float16
+    bfloat16  bfloat16  bfloat16  bfloat16     bfloat16
+    float32   float16   float16   float32      float16     what torch.autocast hands the op: a softmax depth
+    float32   bfloat16  bfloat16  float32      bfloat16    and conv features
+
+Any other pair raises ``B200OpsError`` with status 1. The output has the features' dtype, as the plugin returns its
+input's; the reference's eager path returns float32 because mmdet3d's ``QuickCumsumCuda`` upcasts. FP32 is the reference
+kernel's FFMA chain bit for bit; every 2-byte element is widened to FP32 exactly, FP32 depth is used as loaded, the sum
+is accumulated in FP32 and each 2-byte result rounded once, to nearest even. Both names run the same kernels.
+
+Trainable: the backward returns each gradient in its argument's dtype, ``grad_out`` cast to the features' dtype (FP32
+accumulation, no atomics, the same bits on every run and for every subset of gradients). ``bev_pool_v2_int8`` is the
+INT8 inference form.
 """
 import ctypes
 
@@ -49,13 +59,28 @@ def _extents(depth, feat, ranks):
     return [C, ranks[0].numel(), ranks[3].numel(), depth.numel(), feat.numel() // C]
 
 
+# (depth dtype, feat dtype) -> (forward entry, backward entry, leading feat_dtype argument of the entries)
+_ENTRIES = {
+    (torch.float32, torch.float32): ("b200_bev_pool_f32", "b200_bev_pool_backward_f32", ()),
+    (torch.float16, torch.float16): ("b200_bev_pool_f16", "b200_bev_pool_backward_f16", ()),
+    (torch.bfloat16, torch.bfloat16): ("b200_bev_pool_bf16", "b200_bev_pool_backward_bf16", ()),
+    (torch.float32, torch.float16): ("b200_bev_pool_f32_depth", "b200_bev_pool_backward_f32_depth", (1,)),
+    (torch.float32, torch.bfloat16): ("b200_bev_pool_f32_depth", "b200_bev_pool_backward_f32_depth", (7,)),
+}
+
+
+def _entries(depth, feat):
+    entries = _ENTRIES.get((depth.dtype, feat.dtype))
+    if entries is None:
+        raise _lib.B200OpsError("bev_pool_v2", 1)
+    return entries
+
+
 def _forward(depth, feat, ranks, out_height, out_width):
     depth, feat, ranks = _inputs(depth, feat, ranks)
-    if depth.dtype != feat.dtype or feat.dtype not in (torch.float32, torch.float16):
-        raise _lib.B200OpsError("bev_pool_v2", 1)
+    name, _, lead = _entries(depth, feat)
     out = torch.empty(1, int(out_height), int(out_width), feat.shape[-1], dtype=feat.dtype, device=feat.device)
-    name = "b200_bev_pool_f32" if feat.dtype == torch.float32 else "b200_bev_pool_f16"
-    _lib.call(name, feat.device, depth.data_ptr(), feat.data_ptr(), *(r.data_ptr() for r in ranks),
+    _lib.call(name, feat.device, *lead, depth.data_ptr(), feat.data_ptr(), *(r.data_ptr() for r in ranks),
               *_extents(depth, feat, ranks), int(out_height), int(out_width), out.data_ptr())  # fmt: skip
     return out
 
@@ -72,8 +97,8 @@ def _backward(ctx, grad_out):
     ws = torch.empty(max(P, 1), dtype=torch.int32, device=feat.device)
     dg = torch.empty_like(depth) if need_d else None
     fg = torch.empty_like(feat) if need_f else None
-    name = "b200_bev_pool_backward_f32" if feat.dtype == torch.float32 else "b200_bev_pool_backward_f16"
-    _lib.call(name, feat.device, og.data_ptr(), depth.data_ptr(), feat.data_ptr(), *(r.data_ptr() for r in ranks),
+    _, name, lead = _entries(depth, feat)
+    _lib.call(name, feat.device, *lead, og.data_ptr(), depth.data_ptr(), feat.data_ptr(), *(r.data_ptr() for r in ranks),
               order.data_ptr() if order is not None else None, *_extents(depth, feat, ranks), *ctx.out_hw,
               dg.data_ptr() if need_d else None, fg.data_ptr() if need_f else None, ws.data_ptr(),
               ws.numel() * 4)  # fmt: skip
@@ -111,7 +136,8 @@ _BEVPoolV2_2 = _make("BEVPoolV2TRT2")
 
 def bev_pool_v2(depth, feat, ranks_depth, ranks_feat, ranks_bev, interval_starts, interval_lengths, out_height=128,
                 out_width=128):  # fmt: skip
-    """Plugin BEVPoolV2TRT. Returns [1, out_height, out_width, C] in the inputs' dtype (float32 or float16)."""
+    """Plugin BEVPoolV2TRT. Returns [1, out_height, out_width, C] in the features' dtype; (depth, feat) float32,
+    float16 or bfloat16 pairs, or float32 depth with float16 / bfloat16 features (the module docstring's table)."""
     return _BEVPoolV2.apply(depth, feat, ranks_depth.int(), ranks_feat.int(), ranks_bev.int(), interval_starts.int(),
                             interval_lengths.int(), out_height, out_width)  # fmt: skip
 

@@ -703,11 +703,26 @@ int b200_dcn_supports_format(int pos, const b200_tensor_desc *in_out, int nb_inp
  * depth element referenced by at most one point. Index safety: [s_k, s_k + len_k) is clipped to [0, num_points); an
  * interval whose cell ranks_bev[max(s_k, 0)] is outside [0, out_height*out_width) is dropped, and so is a point whose
  * ranks_depth or ranks_feat is outside its tensor; no input forms an address outside a tensor.
- * Numerics: FP32 = the reference kernel's FFMA chain in point order, bit for bit. FP16 accumulates in FP32 and rounds
- * once. INT8 (channels % 4 == 0, else B200_ERR_UNSUPPORTED): exact int32 sum, one multiply by
+ * Numerics: FP32 = the reference kernel's FFMA chain in point order, bit for bit. FP16 and BF16 accumulate in FP32 and
+ * round once. INT8 (channels % 4 == 0, else B200_ERR_UNSUPPORTED): exact int32 sum, one multiply by
  * scale_depth * scale_feat / scale_out (evaluated in float on the host), saturate, round half away from zero.
  * Pointers of zero-length arrays may be NULL; any other NULL pointer, a pointer not aligned to its element (4 bytes
- * for float and int32, 2 for half) or a negative size is B200_ERR_BAD_PARAM. */
+ * for float and int32, 2 for half and bfloat16) or a negative size is B200_ERR_BAD_PARAM.
+ *
+ * Element types per entry (the `f32_depth` entries take what torch.autocast hands the op: a softmax depth in FP32 and
+ * conv features in FP16 / BF16; feat_dtype = 1 for fp16, 7 for bf16, nvinfer1::DataType's codes, and any other value is
+ * B200_ERR_UNSUPPORTED before anything is launched):
+ *
+ *   entry                    depth   feat, out   depth_grad   out_grad, feat_grad
+ *   _f32                     fp32    fp32        fp32         fp32
+ *   _f16                     fp16    fp16        fp16         fp16
+ *   _bf16                    bf16    bf16        bf16         bf16
+ *   _f32_depth, feat_dtype 1 fp32    fp16        fp32         fp16
+ *   _f32_depth, feat_dtype 7 fp32    bf16        fp32         bf16
+ *
+ * Every 2-byte element is widened to FP32 exactly and FP32 depth is used as loaded; the forward is the FP32 FFMA chain
+ * in point order and each 2-byte result is rounded once, to nearest even. An FP32 depth gradient is not rounded. FP32
+ * depth and its gradient must be 4-byte aligned, every 2-byte tensor 2-byte aligned. */
 int b200_bev_pool_f32(const float *depth, const float *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
                       const int32_t *ranks_bev, const int32_t *interval_starts, const int32_t *interval_lengths,
                       int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
@@ -716,14 +731,23 @@ int b200_bev_pool_f16(const void *depth, const void *feat, const int32_t *ranks_
                       const int32_t *ranks_bev, const int32_t *interval_starts, const int32_t *interval_lengths,
                       int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
                       int out_height, int out_width, void *out, void *stream);
+int b200_bev_pool_bf16(const void *depth, const void *feat, const int32_t *ranks_depth, const int32_t *ranks_feat,
+                       const int32_t *ranks_bev, const int32_t *interval_starts, const int32_t *interval_lengths,
+                       int channels, int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
+                       int out_height, int out_width, void *out, void *stream);
+int b200_bev_pool_f32_depth(int feat_dtype, const float *depth, const void *feat, const int32_t *ranks_depth,
+                            const int32_t *ranks_feat, const int32_t *ranks_bev, const int32_t *interval_starts,
+                            const int32_t *interval_lengths, int channels, int num_points, int num_intervals,
+                            int64_t depth_size, int64_t feat_rows, int out_height, int out_width, void *out,
+                            void *stream);
 int b200_bev_pool_i8(const int8_t *depth, float scale_depth, const int8_t *feat, float scale_feat,
                      const int32_t *ranks_depth, const int32_t *ranks_feat, const int32_t *ranks_bev,
                      const int32_t *interval_starts, const int32_t *interval_lengths, int channels, int num_points,
                      int num_intervals, int64_t depth_size, int64_t feat_rows, int out_height, int out_width,
                      int8_t *out, float scale_out, void *stream);
 
-/* Backward of b200_bev_pool_f32 / _f16, in the input's dtype with FP32 accumulation and no atomics (the same bits on
- * every run and for every subset of gradients asked for):
+/* Backward of b200_bev_pool_f32 / _f16 / _bf16 / _f32_depth, each gradient in its argument's dtype (the table above)
+ * with FP32 accumulation and no atomics (the same bits on every run and for every subset of gradients asked for):
  *   depth_grad[ranks_depth[i]] = sum_c out_grad[cell(i), c] * feat[ranks_feat[i], c]
  *   feat_grad[f, c]            = sum_{i : ranks_feat[i] = f} out_grad[cell(i), c] * depth[ranks_depth[i]]
  * where cell(i) is the cell of the interval that pooled point i (= ranks_bev[i] within the contract); both are zero
@@ -743,6 +767,19 @@ int b200_bev_pool_backward_f16(const void *out_grad, const void *depth, const vo
                                int num_intervals, int64_t depth_size, int64_t feat_rows, int out_height, int out_width,
                                void *depth_grad, void *feat_grad, void *workspace, size_t workspace_size,
                                void *stream);
+int b200_bev_pool_backward_bf16(const void *out_grad, const void *depth, const void *feat, const int32_t *ranks_depth,
+                                const int32_t *ranks_feat, const int32_t *ranks_bev, const int32_t *interval_starts,
+                                const int32_t *interval_lengths, const int32_t *feat_order, int channels,
+                                int num_points, int num_intervals, int64_t depth_size, int64_t feat_rows,
+                                int out_height, int out_width, void *depth_grad, void *feat_grad, void *workspace,
+                                size_t workspace_size, void *stream);
+int b200_bev_pool_backward_f32_depth(int feat_dtype, const void *out_grad, const float *depth, const void *feat,
+                                     const int32_t *ranks_depth, const int32_t *ranks_feat, const int32_t *ranks_bev,
+                                     const int32_t *interval_starts, const int32_t *interval_lengths,
+                                     const int32_t *feat_order, int channels, int num_points, int num_intervals,
+                                     int64_t depth_size, int64_t feat_rows, int out_height, int out_width,
+                                     float *depth_grad, void *feat_grad, void *workspace, size_t workspace_size,
+                                     void *stream);
 
 /* BEVPoolV2TRT[2] (bevPoolPlugin.cpp:71-117): inputs = depth, feat, ranks_depth, ranks_feat, ranks_bev,
  * interval_starts, interval_lengths; output [1, out_height, out_width, C]. Extents come from the descriptors, which

@@ -4,6 +4,10 @@ eager index_select / index_add_ baseline. CUDA events, a warm-up, then the media
 per-call times. Prints the card and its power limit, the workload statistics, the bytes each call moves (computed from
 shapes: HBM-unique bytes and feat bytes gathered from L2, separately), one line per leg and one JSON line at the end.
 
+The BF16 and FP32-depth legs (bf16 / bf16, fp32 depth + fp16 feat, fp32 depth + bf16 feat, forward and backward) are
+timed against FP16 in the same call with their windows alternating (`*_alt` legs, seven windows each), so that the
+comparison does not straddle a change in clocks or in other work on the card.
+
     python scripts/bev_pool_time.py [--iters 200]
 """
 import argparse
@@ -50,6 +54,60 @@ def traffic(depth, feat, ranks, hw, elem):
     out = hw[0] * hw[1] * C * elem
     hbm = depth.numel() * elem + feat.numel() * elem + 3 * P * 4 + 2 * I * 4 + 2 * out
     return {"hbm_unique_MB": round(hbm / 1e6, 1), "l2_gathered_MB": round(P * C * elem / 1e6, 1)}
+
+
+def timed_alternating(legs, iters, windows=7):
+    """{leg: median / min / max per-call µs}, each window of every leg timed in turn, after a warm-up of every leg."""
+    for fn in legs.values():
+        for _ in range(10):
+            fn()
+    torch.cuda.synchronize()
+    per = {k: [] for k in legs}
+    for _ in range(windows):
+        for k, fn in legs.items():
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            for _ in range(iters):
+                fn()
+            b.record()
+            b.synchronize()
+            per[k].append(a.elapsed_time(b) * 1e3 / iters)
+    out = {}
+    for k, v in per.items():
+        v.sort()
+        out[k] = {"median_us": round(v[len(v) // 2], 2), "min_us": round(v[0], 2), "max_us": round(v[-1], 2)}
+    return out
+
+
+# the FP16 baseline and the pairs torch.autocast hands the op: (depth dtype, feat dtype), C entries, leading feat_dtype
+PAIR_LEGS = {"f16_alt": (torch.float16, torch.float16, "b200_bev_pool_f16", "b200_bev_pool_backward_f16", ()),
+             "bf16": (torch.bfloat16, torch.bfloat16, "b200_bev_pool_bf16", "b200_bev_pool_backward_bf16", ()),
+             "f32d_f16": (torch.float32, torch.float16, "b200_bev_pool_f32_depth", "b200_bev_pool_backward_f32_depth",
+                          (1,)),
+             "f32d_bf16": (torch.float32, torch.bfloat16, "b200_bev_pool_f32_depth", "b200_bev_pool_backward_f32_depth",
+                           (7,))}  # fmt: skip
+
+
+def pair_legs(depth, feat, rk, hw):
+    """{leg: call} of the forward and the backward (both gradients) of every PAIR_LEGS pair, through the C ABI: at
+    bevdet_r50 a forward through the autograd binding costs about as much host time as the kernel takes."""
+    legs = {}
+    C = feat.shape[-1]
+    order = torch.sort(rk[1], stable=True).indices.int()
+    ws = torch.empty(rk[0].numel(), dtype=torch.int32, device="cuda")
+    out = torch.empty(1, hw[0], hw[1], C, dtype=torch.float32, device="cuda")  # room for every pair's output
+    for name, (dd, fd, fwd, bwd, lead) in PAIR_LEGS.items():
+        d, f = depth.to(dd).cuda(), feat.to(fd).cuda()
+        gout = torch.randn(1, hw[0], hw[1], C, device="cuda").to(fd)
+        dg, fg = torch.empty_like(d), torch.empty_like(f)
+        legs[f"fwd_{name}"] = lambda d=d, f=f, fwd=fwd, lead=lead: _lib.call(
+            fwd, f.device, *lead, d.data_ptr(), f.data_ptr(), *(r.data_ptr() for r in rk), C, rk[0].numel(),
+            rk[3].numel(), d.numel(), f.numel() // C, hw[0], hw[1], out.data_ptr())  # fmt: skip
+        legs[f"bwd_{name}"] = lambda d=d, f=f, gout=gout, dg=dg, fg=fg, bwd=bwd, lead=lead: _lib.call(
+            bwd, f.device, *lead, gout.data_ptr(), d.data_ptr(), f.data_ptr(), *(r.data_ptr() for r in rk),
+            order.data_ptr(), C, rk[0].numel(), rk[3].numel(), d.numel(), f.numel() // C, hw[0], hw[1], dg.data_ptr(),
+            fg.data_ptr(), ws.data_ptr(), ws.numel() * 4)  # fmt: skip
+    return legs
 
 
 def eager(depth, feat, ranks, hw):
@@ -111,6 +169,7 @@ def main():
         res["fwd_i8"] = timed(lambda: bt.bev_pool_v2_int8(dq, sd, fq, sf, *rk, 0.02, *hw), args.iters)
         if ref is not None:
             res["fwd_i8_ref"] = timed(lambda: ref.forward_int8(dq, sd, fq, sf, rk, 0.02, hw), args.iters)
+        res.update(timed_alternating(pair_legs(depth, feat, rk, hw), args.iters))
         for k, v in res.items():
             if k.startswith(("fwd", "bwd")):
                 print(f"  {name:11s} {k:16s} median {v['median_us']:9.2f} us  (min {v['min_us']}, max {v['max_us']})")
